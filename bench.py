@@ -2,8 +2,12 @@
 """bench.py — waveforms/s of the seist_m_dpk training step (fwd + BCE + bwd + Adam) on (B,3,8192)
 synthetic seismograms; see DESIGN.md §5 for what each JSON key means.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
+
+--dump-outputs DIR writes what the last timed step computed (rank 0) as DIR/<name>.npy: loss, the updated parameters
+and their gradients (flat buffers, float32) and a fixed seeded sample of the model output.  Inputs and initial
+parameters are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -21,6 +25,8 @@ import torch  # noqa: E402
 
 METRIC = "waveforms/sec (B,3,8192) seist_m_dpk fwd+bwd"
 UNIT = "waveforms/s"
+HBM_PEAK_GBS = 3350.0      # H100 SXM data sheet (HBM3); a power-capped card may not reach it
+OUTPUT_SAMPLE = 1 << 20    # model-output elements kept by --dump-outputs (4 MB)
 
 
 def synthetic(n, length, seed, head="dpk"):
@@ -41,7 +47,7 @@ def synthetic(n, length, seed, head="dpk"):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -138,6 +144,21 @@ def _kind_text(kind):
             else "oracle port of the reference step, dropout identity")
 
 
+def dump_outputs(out_dir, trainer):
+    """The last step's results as float32 .npy files: loss, parameters and gradients (the flat buffers the model's
+    parameters and .grad are views of) and OUTPUT_SAMPLE elements of the model output at seeded positions."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    y = trainer.plan.y_out.x.reshape(-1)
+    n = min(OUTPUT_SAMPLE, y.numel())
+    idx = torch.from_numpy(np.sort(np.random.default_rng(0).choice(y.numel(), n, replace=False))).to(y.device)
+    arrays = {"loss": trainer.loss_out.reshape(1), "params": trainer.flat.P, "grads": trainer.flat.G,
+              "output_sample": y[idx]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 def main():
     # stdout carries exactly ONE JSON line: everything else (NCCL banner, library prints) goes to stderr
     real_stdout = os.fdopen(os.dup(1), "w")
@@ -161,7 +182,13 @@ def main():
     ap.add_argument("--cpu-batch", type=int, default=32)
     ap.add_argument("--cpu-steps", type=int, default=12)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's loss, parameters, gradients and an output sample as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the native step computed; the reference arm has no such outputs")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -170,17 +197,16 @@ def main():
     workload = f"{args.model} train step (fwd+BCE+bwd+Adam), batch {args.batch}/GPU x (3,{args.length}) fp32"
     config = {"workload": workload, "model": args.model, "per_gpu_batch": args.batch, "in_samples": args.length,
               "global_batch": args.batch * max(args.gpus, 1), "parallelism": f"dp{max(args.gpus, 1)}",
-              "l2": "per-step working set (GBs of activations) far exceeds the 126 MB L2; no explicit flush",
+              "l2": "per-step working set (GBs of activations) far exceeds the 50 MB L2; no explicit flush",
               "dropout": "reference default rates, counter-based RNG"}
 
     if args.impl == "reference":
         if rank != 0:
             return
-        steps = max(1, min(args.steps, 20))      # bounded sample: ~0.5 s per 32-waveform CPU step
-        warm = max(1, min(args.warmup, 2))
+        steps, warm = args.steps, args.warmup
         rate, secs, kind = reference_step_rate(args.model, args.cpu_batch, args.length, steps, warm, cores)
         config["cpu_sample_batch"] = args.cpu_batch
-        config["workload"] += f"; this arm: the reference's CPU step on {cores} host threads, bounded sample of {args.cpu_batch} waveforms/step"
+        config["workload"] += f"; this arm: the reference's CPU step on {cores} host threads, {args.cpu_batch} waveforms/step"
         line = {"impl": "reference", "metric": METRIC, "value": rate, "unit": UNIT, "n_gpus": args.gpus,
                 "steps": steps, "warmup": warm, "ms_per_step": 1e3 * secs / steps, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config,
@@ -201,13 +227,7 @@ def main():
     dev = torch.device("cuda", local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet"
 
     torch.manual_seed(0)
     model = create_model(args.model, in_channels=3, in_samples=args.length).to(dev)
@@ -238,7 +258,7 @@ def main():
         return float(ms.item())
 
     # ---- device-resident inputs ------------------------------------------------------------------
-    for _ in range(max(args.warmup, 3)):
+    for _ in range(args.warmup):
         trainer.step(x_d, t_d)
     sampler = ClockSampler(local_rank) if rank == 0 else None
     profiling = os.environ.get("SEIST_PROFILE") == "1"     # ncu --profile-from-start off: capture the timed steps only
@@ -251,6 +271,8 @@ def main():
         torch.cuda.profiler.stop()
     clocks = sampler.summary(t0, t1) if sampler else None
     loss_val = float(trainer.loss_out.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer)
     value = args.batch * world * args.steps / (ms / 1e3)
 
     # ---- end to end: pinned host inputs in, loss out, every step ----------------------------------
@@ -288,26 +310,10 @@ def main():
         fam_name, fam = max(fams.items(), key=lambda kv: kv[1]["ms"])
         ach = fam["bytes"] / (fam["ms"] * 1e-3) / 1e9
         top = max((r for r in rows if r.get("family", str(r["kind"])) == fam_name), key=lambda r: r["ms"])
-        # DRAM traffic of the family's largest op from the committed `ncu --set full` capture (profiles/dram_traffic.json:
-        # dram__bytes_read.sum + dram__bytes_write.sum per launch at this batch size), null if not captured
-        traffic = None
-        try:
-            cap = json.load(open(os.path.join(ROOT, "profiles", "dram_traffic.json")))
-            ent = cap.get("ops", {}).get(top["name"])
-            if ent and cap.get("model") == args.model and cap.get("batch") == args.batch:
-                traffic = ent["dram_bytes"]
-        except Exception:
-            pass
-        tensor_pct = None
-        try:
-            tp = json.load(open(os.path.join(ROOT, "profiles", "tensor_pipe.json")))
-            tensor_pct = tp.get("families", {}).get(fam_name)
-        except Exception:
-            pass
         roofline = {"bound": "hbm", "kernel": fam_name, "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                    "frac": ach / hbm_peak, "traffic": traffic, "traffic_op": top["name"], "ms": fam["ms"],
+                    "frac": ach / hbm_peak, "top_op": top["name"], "ms": fam["ms"],
                     "algorithmic_bytes": fam["bytes"], "ops": fam["ops"], "share_of_step": fam["ms"] / tot,
-                    "tflops": fam["flops"] / (fam["ms"] * 1e-3) / 1e12, "tensor_pipe_pct": tensor_pct,
+                    "tflops": fam["flops"] / (fam["ms"] * 1e-3) / 1e12,
                     "peak_source": peak_src,
                     "families": {k: {"ms": round(v["ms"], 3), "share": round(v["ms"] / tot, 4),
                                      "GBps": round(v["bytes"] / (v["ms"] * 1e-3) / 1e9, 1), "ops": v["ops"]}
@@ -325,7 +331,7 @@ def main():
             cpu_baseline = {"value": rate, "unit": UNIT, "cores": cores, "kind": kind,
                             "sample": f"{args.cpu_steps} train steps of {args.cpu_batch} waveforms "
                                       f"({secs:.1f} s; {_kind_text(kind)})"}
-            # informational, same box: the reference's modules under stock PyTorch eager on this B200 (SURVEY 8d)
+            # informational, same GPU: the reference's modules under stock PyTorch eager (SURVEY 8d)
             try:
                 del trainer
                 torch.cuda.empty_cache()
@@ -340,7 +346,7 @@ def main():
         dist.barrier()
     if rank == 0:
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
-                "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps, "higher_is_better": True,
+                "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config,
                 "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": ms_e2e / args.steps,
                         "h2d_bytes_per_step": (x_h.numel() + t_h.numel()) * 4, "d2h_bytes_per_step": 4,

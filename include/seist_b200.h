@@ -1,9 +1,9 @@
 /*
- * seist_b200 — C-ABI of the B200-native SeisT forward/backward hot path.
+ * seist_b200 — C-ABI of the CUDA-native SeisT forward/backward hot path.
  *
  * The reference (senli1073/SeisT) is pure Python/PyTorch and has no FFI of its own; the interfaces
  * these entry points replace are the torch.nn leaf modules its model calls
- * (/root/reference/models/seist.py) — cited per op kind below — plus models/loss.py:32-56 (BCELoss),
+ * (models/seist.py) — cited per op kind below — plus models/loss.py:32-56 (BCELoss),
  * torch.nn.HuberLoss (models/loss.py:3) and the Adam step of training/train.py:304-308,109-111.
  *
  * Conventions: plain pointers and sizes only (no torch types); every pointer is a DEVICE pointer
@@ -201,9 +201,9 @@ uint64_t seist_sizeof_bn(void);
 const char* seist_last_error(void);
 /* number of kernel launches issued by this library since load (bench `gpu_launches`) */
 uint64_t seist_launch_count(void);
-/* name of the kernel family the dispatcher launches for `op` (e.g. "tcconv_fwd(tcgen05+TMA)"); static string */
+/* name of the kernel family the dispatcher launches for `op` (e.g. "pw_fwd(simt)"); static string */
 const char* seist_op_family(const SeistOp* op);
-/* 1 if a tensor-core kernel ever timed out waiting for its MMA completion barrier (bounded spin) */
+/* 1 if a tensor-core kernel ever timed out waiting on one of its mbarriers (bounded spin) */
 int seist_tc_error_flag(void);
 
 /* run ops[0..n) in order on `stream` */

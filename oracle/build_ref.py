@@ -1,12 +1,12 @@
-"""Recipe for `oracle/_ref/`: the UNMODIFIED reference model code, staged so that it travels to the GPU box.
+"""Recipe for `oracle/_ref/`: the UNMODIFIED reference model code, staged beside the package.
 
-TEST / MEASUREMENT INFRASTRUCTURE, not product: only `bench.py` (the `--impl reference` arm, `cpu_baseline`, and the
-informational same-box GPU line) and tests import what this script stages.  `/root/reference` exists only in the build
-container; `oracle/_ref/` is git-ignored (never committed) but not gpurun-ignored, so the staged copy is what lets the
-reference's own `models/seist.py` + `models/loss.py` — default drop rates, torch's own kernels — be timed on the GPU
-box's host cores instead of the oracle port.  Run by `__graft_entry__.build()` when the reference is present:
+MEASUREMENT INFRASTRUCTURE, not product: only `bench.py` (the `--impl reference` arm, `cpu_baseline`, and the
+informational same-GPU line) imports what this script stages.  `oracle/_ref/` is git-ignored (never committed); with it
+the reference's own `models/seist.py` + `models/loss.py` — default drop rates, torch's own kernels — are timed instead
+of the oracle port.  Run by `__graft_entry__.build()`; the checkout is SEIST_REFERENCE_ROOT (default /root/reference),
+and nothing is staged where it does not exist:
 
-    python oracle/build_ref.py            # copies <reference>/models/*.py -> oracle/_ref/models/, timm shim beside it
+    python oracle/build_ref.py            # <checkout>/models/*.py -> oracle/_ref/models/, timm shim beside it
 
 Nothing is edited: files are copied byte for byte and their SHA-256 recorded in oracle/_ref/MANIFEST.json.
 """
@@ -47,7 +47,7 @@ def build() -> bool:
 def import_models():
     """The staged reference `models` package (create_model, BCELoss, ...)."""
     if not available():
-        raise RuntimeError("oracle/_ref is not staged (run oracle/build_ref.py where /root/reference exists)")
+        raise RuntimeError("oracle/_ref is not staged (run oracle/build_ref.py where a reference checkout exists)")
     if OUT not in sys.path:
         sys.path.insert(0, OUT)
     import models as ref_models

@@ -2,13 +2,13 @@
 model's probability traces, and the precision/recall/residual counters built from them.
 
 Restates, in numpy, for the reference's default configuration (mpd > 1, rising edges, no valley / kpsh / threshold):
-  * `_detect_peaks`  — /root/reference/training/postprocess.py:15-111 (BMC detect_peaks + top-k), called by
+  * `_detect_peaks`  — training/postprocess.py:15-111 (BMC detect_peaks + top-k), called by
   * `_pick_phase`    — :161-193 (pads to `topk` with -1e7),
   * `_detect_event`  — :114-158, which calls obspy.signal.trigger.trigger_onset(x, thr, thr).  obspy is a third-party
-                       dependency absent from /root/reference and from this image (requirements.txt pins obspy==1.4.0);
+                       dependency absent from the reference (requirements.txt pins obspy==1.4.0);
                        with equal on/off thresholds its published algorithm returns the maximal runs of x > thr as
                        inclusive [on, off] index pairs.  PARITY UNPINNED for this one function (no obspy to run);
-  * `Metrics.compute` counters for the tasks ppk / spk / det — /root/reference/utils/metrics.py:141-247.
+  * `Metrics.compute` counters for the tasks ppk / spk / det — utils/metrics.py:141-247.
 `pick_phase` IS pinned: tests/test_cpu_postprocess.py executes the reference's own `_detect_peaks` source (extracted from
 the file with `ast`, nothing else of that module imports here) on random and crafted traces and compares index for index.
 Tie rule: for EQUAL peak heights the reference's order is unspecified (`np.argsort` defaults to an unstable, on x86 SIMD,

@@ -1,5 +1,5 @@
 """CPU oracle (TEST INFRASTRUCTURE) for the input side of SURVEY §8f-3: per-trace normalisation and the soft labels of
-the dpk task, restated in numpy from /root/reference/training/preprocess.py:
+the dpk task, restated in numpy from the reference's training/preprocess.py:
 
   * `normalize`        — `DataPreprocessor._normalize` :224-242 (mean removal per channel, then max or std scaling;
                          note: `max` is the signed maximum, not max |x|, and a zero scale is replaced by 1);

@@ -1,7 +1,7 @@
-"""Import the UNMODIFIED reference from /root/reference (exists only in the build container).
+"""Import the UNMODIFIED reference from a SeisT checkout (SEIST_REFERENCE_ROOT, default /root/reference).
 
-Used to (a) pin oracle/seist_ref.py against the real code and (b) generate tests/golden fixtures.
-Never used on the GPU box (the path does not exist there) — callers must check `available()`.
+Used only to generate the tests/golden fixtures (tests/golden/make_golden.py); nothing in the tests, the
+benchmark or the package needs a reference checkout.
 """
 import os
 import sys
@@ -11,7 +11,7 @@ _SHIM = os.path.join(os.path.dirname(os.path.abspath(__file__)), "timm_shim")
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REF_ROOT, "models", "seist.py"))
+    return bool(REF_ROOT) and os.path.isfile(os.path.join(REF_ROOT, "models", "seist.py"))
 
 
 def import_reference_models():

@@ -1,4 +1,4 @@
-"""seist_b200 — B200-native (sm_100a) implementation of the SeisT forward/backward hot path.
+"""seist_b200 — CUDA-native (sm_90a, H100) implementation of the SeisT forward/backward hot path.
 
 Public surface mirrors the reference's (senli1073/SeisT):
   seist_b200.models   — register_model / create_model / get_model_list / save_checkpoint /

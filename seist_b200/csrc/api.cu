@@ -44,16 +44,10 @@ int launch_res_bwd4(const SeistOp& op, cudaStream_t s, int sm_count);
 bool bww_eligible(const SeistOp& op);
 int launch_bww_any(const SeistOp& op, cudaStream_t s, int sm_count);
 bool convk_eligible(const SeistOp& op);
-bool pw_tc_eligible(const SeistOp& op);
-int launch_pw_tc_fwd(const SeistOp& op, cudaStream_t s, int sm_count);
-int pw_tc_error_flag();
-bool bww_tc_eligible(const SeistOp& op);
-int launch_bww_tc(const SeistOp& op, cudaStream_t s, int sm_count);
 bool bwwk_eligible(const SeistOp& op);
 int launch_grad_combine(const SeistOp& op, cudaStream_t s, int sm_count);
 bool convk_bwd_data_eligible(const SeistOp& op);
 int launch_bwwk(const SeistOp& op, cudaStream_t s, int sm_count);
-int bww_tc_error_flag();
 int launch_convk_fwd(const SeistOp& op, cudaStream_t s);
 int launch_convk_bwd_data(const SeistOp& op, cudaStream_t s);
 int launch_bn_prepare(const SeistOp& op, bool fwd, cudaStream_t s);
@@ -62,10 +56,6 @@ bool tcconv_eligible(const SeistOp& op, int mode);
 int launch_tcconv(const SeistOp& op, int mode, cudaStream_t s, int sm_count);
 int tcconv_error_flag();
 
-// tensor-core (tcgen05) paths (pw_tc.cu forward, bww_tc.cu weight gradient): validated against the interpreter
-// (tests/test_gpu_ops.py::test_tcgen05_kernels_match_interpreter) but, since the SIMT kernels moved to FFMA2 and
-// 4 CTAs/SM, slower than them on every op of the model family (profiles/r1_tc_vs_simt.txt) - opt-in:
-// SEIST_TC=1 every eligible op, SEIST_TC=2 the former heuristic (GELU-input / wide contractions), default never.
 // integer tuning knob, read from the environment on every call (launch time only; graphs replay the captured choice)
 int env_knob(const char* name, int def) {
   const char* e = std::getenv(name);
@@ -76,62 +66,33 @@ int bww_waves() {
   if (v < 0) { const char* e = std::getenv("SEIST_BWW_WAVES"); v = (e && e[0] >= '1' && e[0] <= '4') ? e[0] - '0' : 2; }
   return v;
 }
-static int tc_mode() {
-  static int v = -1;
-  if (v < 0) { const char* e = std::getenv("SEIST_TC"); v = !e ? 0 : (e[0] == '1' ? 1 : (e[0] == '2' ? 2 : 0)); }
-  return v;
-}
 // sliding-window weight-gradient kernel for k > 1 (bwwk.cu); SEIST_BWWK=0 falls back to the row-tiled kernel (A/B runs)
 static int bwwk_mode() {
   static int v = -1;
   if (v < 0) { const char* e = std::getenv("SEIST_BWWK"); v = (e && e[0] == '0') ? 0 : 1; }
   return v;
 }
-static bool use_tc(const SeistOp& op) {
-  const int mode = tc_mode();
-  if (mode == 0 || !pw_tc_eligible(op)) return false;
-  if (mode == 1) return true;
-  bool gelu = false;
-  for (int i = 0; i < op.n_in; ++i) gelu = gelu || op.in[i].act == SEIST_ACT_GELU;
-  return (gelu && op.Cin >= 32 && op.Cout >= 16) || (op.Cin >= 64 && op.Cout >= 32);
-}
-
-// Tensor-core dispatch.  Measured on B200 at the bench configuration (profiles/r2_tc_vs_simt.txt): the warp-specialised
-// tcgen05 + TMA engine (tcconv.cu) beats the FFMA2 SIMT kernels where the contraction is wide or has taps to amortise
-// its per-element transform / epilogue cost (k-tap convolutions of the encoder stages at L <= 512, 1x1 convolutions with
-// >= 64 reduction channels), and loses on the narrow, long layers (stem, stage 0, head) where a SIMT thread does only
-// Cout/2 packed FMAs per input element.  SEIST_TCC: unset/"auto" = that rule, "1" = every eligible op (tests), "0" = never.
+// Tensor-core convolution engine (tcconv.cu: wgmma + TMA, 3 x TF32) for stride-1 forward / data-gradient convs.  Measured
+// op by op on H100 at the bench configuration (seist_m_dpk, B = 512, engine forced vs SIMT kernels): it wins on the
+// up-sampled head convs with >= 32 input channels, the k-tap convs of encoder stages 1-3 (forward at L <= 512 with >= 16
+// reduction channels, data gradient at L <= 256 with >= 32) and the forward 1x1 convs with >= 64 reduction channels at
+// L <= 256; everywhere else (stem, stage 0, the long head layers, most 1x1 data gradients) the SIMT kernels are faster.
+// SEIST_TCC: unset = that rule, "1" = every eligible op (tests), "0" = never.
 static int tcc_mode() {
   static int v = -1;
   if (v < 0) { const char* e = std::getenv("SEIST_TCC"); v = !e ? 2 : (e[0] == '0' ? 0 : (e[0] == '1' ? 1 : 2)); }
   return v;
 }
 static bool tcc_auto(const SeistOp& op, int mode) {
-  const int Kd = mode == 0 ? op.Cin : op.Cout, Nd = mode == 0 ? op.Cout : op.Cin;
-  // dpk head forward (x2 up-sampled operand, k = 7 dense taps): measured wins for the 64->32 and 32->24 layers (0.277 -> 0.191,
-  // 0.274 -> 0.161 ms); 96->64 does not fit its 344 KB of split weights in shared memory (re-staged per tile: 0.438 -> 0.460)
-  // and the 16/24-channel layers at L >= 2048 are transform-bound (gpurun_out/op_times_r2l.json)
-  if (op.up_src_L > 0) return mode == 0 && Kd >= 32 && Kd <= 64;
-  if (op.k > 1) return op.L_out <= 512 && Kd >= 8 && Nd >= 8;
-  if (mode == 0) return Kd >= 64 && Nd >= 48;
-  return Kd >= 96 && Nd >= 96;
+  const int Kd = mode == 0 ? op.Cin : op.Cout;
+  if (op.up_src_L > 0) return mode == 0 && Kd >= 32;
+  if (op.k > 1) return mode == 0 ? (op.L_out <= 512 && Kd >= 16) : (op.L_out <= 256 && Kd >= 32);
+  return mode == 0 && Kd >= 64 && op.L_out <= 256;
 }
 static bool use_tcc(const SeistOp& op, int mode) {
   const int m = tcc_mode();
   if (m == 0 || !tcconv_eligible(op, mode)) return false;
   return m == 1 || tcc_auto(op, mode);
-}
-// weight gradient of wide 1x1 convolutions on tcgen05 (bww_tc.cu).  Timed alone it wins from 64 reduction channels up
-// (37 ops of seist_m_dpk: 2.42 ms against 2.9 ms for the SIMT kernel), but the weight gradients run on the side lane
-// CONCURRENTLY with the data-gradient chain, and there its 148 x 2 CTAs with their large shared-memory / TMEM footprint
-// displace more main-lane CTAs than they save: whole step 36.81 ms with it, 36.44 ms without (gpurun sweep_i, sweep_j).
-// What counts for a side-lane kernel is the step, so it is opt-in: SEIST_BWW_TC=1 (rule below), SEIST_TC=1 (every op).
-static bool use_bww_tc(const SeistOp& op) {
-  if (!bww_tc_eligible(op)) return false;
-  const int m = tc_mode();
-  if (m == 1) return true;
-  if (!env_knob("SEIST_BWW_TC", 0)) return false;
-  return op.Cin >= 64 && op.Cout >= 32 && op.L_out <= 256;
 }
 
 static int sm_count() {
@@ -139,7 +100,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g_sm_count <= 0)
-      g_sm_count = 148;
+      g_sm_count = 132;
   }
   return g_sm_count;
 }
@@ -156,14 +117,14 @@ static int validate_conv(const SeistOp& op) {
 
 // which kernel family serves an op (also reported to the bench: `seist_op_family`)
 enum Family {
-  F_NONE = 0, F_TCCONV_FWD, F_TCCONV_BWD_DATA, F_PW_TC_FWD, F_PW_FWD, F_CONVK_FWD, F_CONV_FWD, F_PW_BWD_DATA, F_CONVK_BWD_DATA,
-  F_CONV_BWD_DATA, F_BWW_TC, F_BWWK, F_BWW, F_CONV_BWD_W, F_RES_BWD, F_RES_BWD4, F_ATT_FWD, F_ATT_BWD_Q, F_ATT_BWD_KV, F_HEADVEC_FWD,
+  F_NONE = 0, F_TCCONV_FWD, F_TCCONV_BWD_DATA, F_PW_FWD, F_CONVK_FWD, F_CONV_FWD, F_PW_BWD_DATA, F_CONVK_BWD_DATA,
+  F_CONV_BWD_DATA, F_BWWK, F_BWW, F_CONV_BWD_W, F_RES_BWD, F_RES_BWD4, F_ATT_FWD, F_ATT_BWD_Q, F_ATT_BWD_KV, F_HEADVEC_FWD,
   F_HEADVEC_BWD, F_BN_FINALIZE_FWD, F_BN_FINALIZE_BWD, F_BN_PREPARE_FWD, F_BN_PREPARE_BWD, F_STEM_COMPOSE_FWD, F_STEM_COMPOSE_BWD,
   F_GRAD_COMBINE, F_ZERO
 };
 static const char* kFamilyName[] = {
-  "none", "tcconv_fwd(tcgen05+TMA)", "tcconv_bwd_data(tcgen05+TMA)", "pw_tc_fwd(tcgen05)", "pw_fwd(simt)", "convk_fwd(simt)",
-  "conv_fwd(simt)", "pw_bwd_data(simt)", "convk_bwd_data(simt)", "conv_bwd_data(simt)", "bww_tc(tcgen05)", "bwwk(simt)", "bww(simt)",
+  "none", "tcconv_fwd(wgmma+TMA)", "tcconv_bwd_data(wgmma+TMA)", "pw_fwd(simt)", "convk_fwd(simt)",
+  "conv_fwd(simt)", "pw_bwd_data(simt)", "convk_bwd_data(simt)", "conv_bwd_data(simt)", "bwwk(simt)", "bww(simt)",
   "conv_bwd_w(simt)", "res_bwd", "res_bwd4", "att_fwd", "att_bwd_q", "att_bwd_kv", "headvec_fwd", "headvec_bwd", "bn_finalize_fwd",
   "bn_finalize_bwd", "bn_prepare_fwd", "bn_prepare_bwd", "stem_compose_fwd", "stem_compose_bwd", "grad_combine", "zero"
 };
@@ -172,7 +133,6 @@ static Family choose(const SeistOp& op) {
   switch (op.kind) {
     case SEIST_OP_CONV_FWD:
       if (use_tcc(op, 0)) return F_TCCONV_FWD;
-      if (use_tc(op)) return F_PW_TC_FWD;
       if (pw_eligible(op)) return F_PW_FWD;
       return convk_eligible(op) ? F_CONVK_FWD : F_CONV_FWD;
     case SEIST_OP_CONV_BWD_DATA:
@@ -180,7 +140,6 @@ static Family choose(const SeistOp& op) {
       if (pw_eligible(op)) return F_PW_BWD_DATA;
       return convk_bwd_data_eligible(op) ? F_CONVK_BWD_DATA : F_CONV_BWD_DATA;
     case SEIST_OP_CONV_BWD_W:
-      if (use_bww_tc(op)) return F_BWW_TC;
       if (bwwk_mode() && bwwk_eligible(op)) return F_BWWK;
       return bww_eligible(op) ? F_BWW : F_CONV_BWD_W;
     case SEIST_OP_RES_BWD: return (op.L_out & 3) ? F_RES_BWD : F_RES_BWD4;
@@ -209,14 +168,12 @@ static int run_one(const SeistOp& op, cudaStream_t s) {
   switch (choose(op)) {
     case F_TCCONV_FWD: return launch_tcconv(op, 0, s, sm_count());
     case F_TCCONV_BWD_DATA: return launch_tcconv(op, 1, s, sm_count());
-    case F_PW_TC_FWD: return launch_pw_tc_fwd(op, s, sm_count());
     case F_PW_FWD: return launch_pw_fwd(op, s, sm_count());
     case F_CONVK_FWD: return launch_convk_fwd(op, s);
     case F_CONV_FWD: return launch_conv_fwd(op, s);
     case F_PW_BWD_DATA: return launch_pw_bwd_data(op, s, sm_count());
     case F_CONVK_BWD_DATA: return launch_convk_bwd_data(op, s);
     case F_CONV_BWD_DATA: return launch_conv_bwd_data(op, s);
-    case F_BWW_TC: return launch_bww_tc(op, s, sm_count());
     case F_BWWK: return launch_bwwk(op, s, sm_count());
     case F_BWW: return launch_bww_any(op, s, sm_count());
     case F_CONV_BWD_W: return launch_conv_bwd_w(op, s, sm_count());
@@ -256,7 +213,7 @@ uint64_t seist_sizeof_bn(void) { return sizeof(SeistBN); }
 const char* seist_last_error(void) { return seist::g_err; }
 uint64_t seist_launch_count(void) { return seist::g_launches.load(); }
 const char* seist_op_family(const SeistOp* op) { return op ? seist::kFamilyName[seist::choose(*op)] : "none"; }
-int seist_tc_error_flag(void) { return seist::pw_tc_error_flag() | seist::bww_tc_error_flag() | seist::tcconv_error_flag(); }
+int seist_tc_error_flag(void) { return seist::tcconv_error_flag(); }
 
 // fork/join events of seist_plan_run2, one pool per device (events belong to the device that was current at creation)
 static std::vector<cudaEvent_t> g_events[64];

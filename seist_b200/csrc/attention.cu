@@ -13,7 +13,7 @@ constexpr int KV_CHUNK = 128;
 
 // Shared rows are stored per key / query: [j][K(E) | V(E)] (pitch 2E+4 floats keeps 16-byte alignment and
 // spreads the transposing stores over 8 bank groups), so the thread that owns a query column reads the whole
-// key as E/4 broadcast 16-byte loads and contracts it with FFMA2 over (even, odd) feature pairs.
+// key as E/4 broadcast 16-byte loads and contracts it over (even, odd) feature pairs (fma2).
 template <int E>
 struct AttRow {
   static constexpr int PITCH = 2 * E + 4;
@@ -108,7 +108,7 @@ __global__ void __launch_bounds__(ATT_NT) att_fwd_kernel(const __grid_constant__
           const float r = __expf(m - s);
           den *= r;
 #pragma unroll
-          for (int e = 0; e < E / 2; ++e) o[e] = __fmul2_rn(o[e], dup2(r));
+          for (int e = 0; e < E / 2; ++e) o[e] = mul2(o[e], dup2(r));
           m = s;
         }
         const float p = __expf(s - m);

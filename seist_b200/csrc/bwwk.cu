@@ -15,8 +15,8 @@
 // laid out as TG = TGM*nci tile coordinates x PG sample groups; the sample groups are folded through shared
 // memory at the end, one float atomic per dW element per CTA.
 //
-// FFMA2: the gacc rows are parked in shared memory interleaved in channel pairs ({g[2r][s], g[2r+1][s]}), so a
-// 16-byte load yields two aligned (even, odd channel) register pairs; each FFMA2 multiplies such a pair with one
+// fma2: the gacc rows are parked in shared memory interleaved in channel pairs ({g[2r][s], g[2r+1][s]}), so a
+// 16-byte load yields two aligned (even, odd channel) register pairs; each fma2 multiplies such a pair with one
 // broadcast window sample: 8*K packed FMAs per quad instead of 16*K scalar ones.
 #include <algorithm>
 #include "common.cuh"
@@ -250,7 +250,7 @@ static int launch_bwwk_t(const SeistOp& op, cudaStream_t s, int sm_count) {
                 (op.up_src_L > 0 ? sizeof(float) * (size_t)CI_B * (width + 4) : 0) + 16;
   // raw planes of the asynchronous gacc staging (x, dxd next to du) - unless they would cost a resident CTA
   int gx_off = 0;
-  if (env_knob("SEIST_ASYNC", 7) & 8) {   // measured: bww 8.66 -> 8.40 ms with it, this kernel 6.64 -> 6.77 (gpurun sweep_l): off here
+  if (env_knob("SEIST_ASYNC", 7) & 8) {   // opt-in: it helps the row-tiled kernel more than this one
     const bool has_bn = op.out.bn >= 0 && op.out.g != nullptr;
     const bool need_x = has_bn || op.out_act == SEIST_OUT_SIGMOID;
     const int planes = (need_x ? 1 : 0) + ((has_bn && op.out_dxd != nullptr) ? 1 : 0);

@@ -1,4 +1,4 @@
-// Shared device helpers for the seist_b200 kernels (sm_100a).
+// Shared device helpers for the seist_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,15 +19,18 @@ int check_launch(const char* what);
 void set_error(const char* msg);
 
 // ---- math -------------------------------------------------------------------------------------
-// packed fp32 FMA (sm_100 FFMA2, fma.rn.f32x2): two IEEE fused multiply-adds per issue slot, bit-identical to
-// two scalar fmaf.  Measured on B200 (tools/ffma2_probe.cu): 65.7 TFLOP/s vs 46.7 for scalar FFMA.
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
+// Two-lane fp32 helpers.  Hopper has no packed fp32 instructions, so each lane is one scalar IEEE operation; the
+// _rn intrinsics keep the compiler from contracting a multiply and an add into an FMA, so the kernels compute exactly
+// the sequence of roundings written here.
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 __device__ __forceinline__ float2 dup2(float v) { return make_float2(v, v); }
 
 // exact-erf GELU (nn.GELU(), models/seist.py:640) with erf by Abramowitz & Stegun 7.1.26: |abs error| <= 1.5e-7, i.e. at the
 // level of fp32 rounding of erff itself, in 1 rcp + 1 ex2 + 7 fma instead of erff's ~40 instructions (two polynomial
-// branches).  GELU / GELU' sit in the load prologue of every kernel that consumes an activated view, where they were 25-60 %
-// of the executed instructions of the narrow layers.
+// branches).  GELU / GELU' sit in the load prologue of every kernel that consumes an activated view, where they are a large
+// share of the executed instructions of the narrow layers.
 __device__ __forceinline__ float fast_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -54,15 +57,12 @@ __device__ __forceinline__ float gelu_grad_f(float x) {
   const float pdf = 0.39894228040143267794f * fast_ex2(-0.72134752044448170368f * x * x);
   return fmaf(x, pdf, cdf);
 }
-// ---- packed (two elements per instruction) versions: FMUL2 / FADD2 / FFMA2 ----------------------------------------------
-// The element-wise prologue / epilogue math (BN affine, GELU, GELU', BN-backward combine) was 40 % of the executed
-// instructions of the narrow 1x1 kernels as scalar FMUL / FFMA / FADD (ncu, profiles/r2_pw_bwd_data_mix.txt) against 11 %
-// for the contraction itself.  The packed forms issue half as many instructions; only |.|, copysign and the two MUFU per
-// element stay scalar.  gelu2 is bit-identical to gelu_f per lane (same operations in the same order, the polynomial
-// negated coefficient by coefficient); gelu_grad2 shares erf's exponential with the density term
-// (exp(-z^2), z = x / sqrt 2, is exp(-x^2 / 2)), one MUFU less than gelu_grad_f and equal to it within 2 ulp.
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return __fadd2_rn(a, b); }
+// ---- two-element versions of the element-wise math ------------------------------------------------------------------
+// gelu2 is bit-identical to gelu_f per lane (same operations in the same order, the polynomial negated coefficient by
+// coefficient); gelu_grad2 shares erf's exponential with the density term (exp(-z^2), z = x / sqrt 2, is exp(-x^2 / 2)),
+// one MUFU less than gelu_grad_f and equal to it within 2 ulp.
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 // erf(z) per lane; e = exp(-z^2) is returned as well
 __device__ __forceinline__ float2 erf2(float2 z, float2& e) {
   const float2 a = make_float2(fabsf(z.x), fabsf(z.y));
@@ -130,8 +130,7 @@ __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + __ex
 
 // ---- asynchronous global -> shared copies (LDGSTS) ---------------------------------------------------------------------
 // Staging loops of the form "load, transform, store to shared" expose one memory latency per iteration unless the compiler
-// can batch the loads (it cannot across the conditional GELU); ncu showed 35-50 % of the stall samples of the weight-
-// gradient / k-tap kernels on the first use of such a load.  The kernels therefore copy the RAW operands with cp.async
+// can batch the loads (it cannot across the conditional GELU).  The kernels therefore copy the RAW operands with cp.async
 // (every copy of a tile in flight at once, no registers held) and the issuing thread transforms its own elements in place
 // after cp.async.wait_group (which orders a thread's own copies: no barrier between copy and transform).
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -27,7 +27,7 @@ struct CkWin {
 };
 
 // acc[c][j] += sum_t w[t][c] * win[j*S + t] for one reduction channel
-// channel pairs ride the two lanes of FFMA2; ck_acc reads channel c, sample j of a [4][4] pair tile
+// channel pairs ride the two lanes of fma2; ck_acc reads channel c, sample j of a [4][4] pair tile
 __device__ __forceinline__ float ck_acc(const float2 (&acc)[4][4], int c, int j) { return (c & 1) ? acc[c >> 1][j].y : acc[c >> 1][j].x; }
 
 template <int K, int S>
@@ -301,7 +301,7 @@ __global__ void __launch_bounds__(CK_NT, 3) convk_bwd_data_kernel(const __grid_c
       const int co = co_grp + co0 + r;
       const OutGradCoef kc = out_grad_coef(op, co);
       float* d = zb + r * pitch;
-      for (int pos = lane; pos < pos_hi; pos += 32) {     // (scalar: the packed form measured slower here)
+      for (int pos = lane; pos < pos_hi; pos += 32) {     // (scalar)
         if (pos < pos_lo) continue;
         float g = d[pos];
         if (need_x) {
@@ -566,9 +566,8 @@ static int pick_wc(int channels) { return channels > 32 ? 8 : (channels > 16 ? 4
 static int ck_pick_nbuf(size_t bytes1, size_t bytes2) {
   const int knob = env_knob("SEIST_CK_NBUF", 0);
   if (knob == 1 || knob == 2) return bytes2 > 220 * 1024 ? 1 : knob;
-  // measured on B200 (gpurun sweep_b): the second stage costs a resident CTA on most layers of the model family and
-  // loses more than the prefetch wins (convk_fwd 4.16 -> 4.46 ms, convk_bwd_data 4.77 -> 4.89 ms per step): two stages
-  // only where they are free
+  // the second stage costs a resident CTA on most layers of the model family, which loses more than the prefetch wins:
+  // two stages only where they are free
   auto ctas = [](size_t b) { return (int)std::min<size_t>(3, (227 * 1024) / (b + 1024)); };
   return (ctas(bytes2) >= ctas(bytes1) && bytes2 <= 220 * 1024) ? 2 : 1;
 }

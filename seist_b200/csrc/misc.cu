@@ -342,7 +342,7 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const float* __restrict__ p
 static int ew_grid(int64_t total) {
   int64_t g = (total + 256 * 8 - 1) / (256 * 8);
   if (g < 1) g = 1;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   return (int)g;
 }
 

@@ -61,9 +61,8 @@ __device__ __forceinline__ PwChan make_chan(const SeistOp& op, int ci, bool want
   return c;
 }
 
-// (scalar on purpose: the packed FMUL2 / FADD2 forms of this element-wise math measured SLOWER in the latency-bound 1x1
-// kernels - pw_bwd_data 8.95 -> 9.74 ms, pw_fwd 4.61 -> 4.82 ms per step - while they help the staged kernels, where the
-// transform is a separate pass over shared memory; gpurun sweep_d)
+// (scalar on purpose: the latency-bound 1x1 kernels interleave this math with their loads; the staged kernels, where the
+// transform is a separate pass over shared memory, use the two-lane forms)
 __device__ __forceinline__ float4 apply_view(float4 v, float sc, float sh, int act) {
   v.x = fmaf(sc, v.x, sh);
   v.y = fmaf(sc, v.y, sh);
@@ -113,8 +112,7 @@ __device__ __forceinline__ float4 pw_load_pooled(const float* src, int P, float 
 // Backward of AvgPool1d(P) + MaxPool1d(P) in front of a 1x1 conv (reference models/seist.py:62-76) for one target channel
 // of one thread: NJ pooled gradients gq[0..NJ) go to their NJ*P contiguous source samples as g * (1/P + [first arg max of the
 // BN-applied values]).  The source samples are read and written with 16-byte accesses and the arg max is found in
-// registers; the former version walked them with P scalar loads + P/2 float2 loads and stores per pooled sample (5x the
-// time of a plain target of the same size, profiles/r2_op_times_final.json).  s1 / s2: BN-backward sums of the targets.
+// registers instead of P scalar loads + P/2 float2 loads and stores per pooled sample.  s1 / s2: BN-backward sums of the targets.
 template <int P, int NJ>
 __device__ __forceinline__ void pool_route_part(const PwChan& c, const float4* xs, float4* gs, const float* gq, float& s1,
                                                 float& s2) {
@@ -310,7 +308,7 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_fwd_kernel(const __grid_constant_
     const bool ok = f < NQ;
     const int n = ok ? (int)(f / LQ) : 0;
     const int l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
-    float2 acc[COUT_T / 2][4];   // [channel pair][sample]: .x = even channel, .y = odd channel (FFMA2 lanes)
+    float2 acc[COUT_T / 2][4];   // [channel pair][sample]: .x = even channel, .y = odd channel (fma2 lanes)
 #pragma unroll
     for (int c = 0; c < COUT_T / 2; ++c)
 #pragma unroll
@@ -557,7 +555,7 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
     const int n = ok ? (int)(f / LQ) : 0;
     const int l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
     const float pf = path_factor(op, seed, n) * alpha_factor(op, seed, n);
-    float2 acc[CI_T / 2][4];   // [target-channel pair][sample] (FFMA2 lanes = even / odd channel)
+    float2 acc[CI_T / 2][4];   // [target-channel pair][sample] (fma2 lanes = even / odd channel)
 #pragma unroll
     for (int c = 0; c < CI_T / 2; ++c)
 #pragma unroll
@@ -845,7 +843,7 @@ static thread_local int tl_sm_count = 0;
 static thread_local long long tl_groups = 0;
 template <typename K>
 static void pw_persist(K kernel, size_t smem, dim3& grid, int& G) {
-  if (!env_knob("SEIST_PW_PERSIST", 0) || tl_sm_count <= 0) return;   // measured: pw_fwd 4.55 -> 4.47 but pw_bwd_data 8.35 -> 8.77 ms per step (gpurun sweep_h): opt-in
+  if (!env_knob("SEIST_PW_PERSIST", 0) || tl_sm_count <= 0) return;   // opt-in
   int nb = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, PW_NT, smem) != cudaSuccess || nb < 1) return;
   long long gx = (long long)nb * tl_sm_count / grid.y;
@@ -946,7 +944,7 @@ static int pw_bwdd_sel(const SeistOp& op, cudaStream_t s, dim3 grid, size_t smem
     if (op.in[i].bn >= 0 || op.in[i].act == SEIST_ACT_GELU) pre |= 1;
     if (op.in[i].accum) pre |= 2;
   }
-  pre &= env_knob("SEIST_PW_PRE", 0);   // measured: the prefetch planes cost a resident CTA and lose (8.95 -> 9.95 ms per step, gpurun sweep_c): opt-in
+  pre &= env_knob("SEIST_PW_PRE", 0);   // the prefetch planes cost a resident CTA: opt-in
   const int sel = (op.p_elem > 0.f ? 2 : 0) | (any_gelu(op) ? 1 : 0);
   switch (sel) {
     case 0: return pw_bwdd_go<CIT, false, false>(op, s, grid, smem, G, pre);
@@ -1051,7 +1049,7 @@ constexpr int BW_NT = 256;
 template <int CO_B, int R_B, bool K1, int BW_PC>
 __global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ SeistOp op, const int nci_max, const int async_in, const int gx_off) {
   constexpr int BW_PITCH = BW_PC + 4;   // input row pitch (floats), keeps 16-byte alignment
-  constexpr int BW_GP = 2 * BW_PC + 8;  // gacc channel-PAIR row pitch: g_s[pr][2*s + half] (FFMA2 operand pairs)
+  constexpr int BW_GP = 2 * BW_PC + 8;  // gacc channel-PAIR row pitch: g_s[pr][2*s + half] (fma2 operand pairs)
   extern __shared__ __align__(16) unsigned char sm_raw[];
   constexpr int TGM = CO_B / 4, TGN = R_B / 8, TG = TGM * TGN, PG = BW_NT / TG;
   static_assert(TG <= BW_NT && BW_NT % TG == 0, "bad tile");
@@ -1126,9 +1124,8 @@ __global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ S
     const int l0 = (tile - n * chunks_per_n) * BW_PC;
     const float pf = path_factor(op, seed, n) * alpha_factor(op, seed, n);
     // ---- conv-input rows, k = 1 fast path: raw 16-byte asynchronous copies, ALL in flight at once and behind the
-    // gacc loads below; every thread later transforms its own quads in place (no barrier in between).  The former
-    // load -> transform -> store loop exposed one memory latency per quad (ncu: 37 % of the kernel's stall samples
-    // on the first use of that load)
+    // gacc loads below; every thread later transforms its own quads in place (no barrier in between).  A
+    // load -> transform -> store loop would expose one memory latency per quad
     const bool in_async = K1 && vec && plain && async_in;
     if (in_async) {
       for (int idx = tid; idx < nci * QPR; idx += BW_NT) {

@@ -1,4 +1,4 @@
-// Convolution forward / data-gradient on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// Convolution forward / data-gradient on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 //   forward        out[co][l] = sum_{ci,t} W[co][ci][t] * f(in[ci])[l*1 + t - pad]        (nn.Conv1d, models/seist.py:86..546)
 //   data gradient  dIn[ci][p] = sum_{co,t} W[co][ci][t] * gacc[co][p + pad - t]            (its autograd transpose)
@@ -6,21 +6,22 @@
 // Both are the same GEMM per 128-sample tile:  D[M = 128 samples][N = result channels] += A_t[M][K] * B_t[N][K]^T summed
 // over the k taps t, where A_t is the SAME shared-memory panel read at a row offset of t samples:
 //
-//   panel layout (UMMA K-major, no swizzle):  [channel/4][row][channel%4]  (16 bytes = 4 reduction channels of one sample)
+//   panel layout (K-major, no swizzle):  [channel/4][row][channel%4]  (16 bytes = 4 reduction channels of one sample)
 //   a core matrix (8 rows x 16 B) of channel-quad q starting at ANY row r0 is the contiguous 128 bytes at q*pitch + r0*16,
 //   so the descriptor of tap t is just  start += 16*t  (LBO = pitch between channel quads, SBO = 128 between 8-row groups).
-//   No im2col copy, no weight expansion: k * ceil(K/8) MMAs of 128 x N x 8 per tile and precision pass.
+//   No im2col copy, no weight expansion: k * ceil(K/8) MMA steps per tile and precision pass.
 //
-// Warp roles (one persistent CTA per SM, 576 threads):
-//   warp 17      TMA producer: cp.async.bulk.tensor boxes {rows, 8 channels} of the raw fp32 operand tensors -> raw ring
+// Warp roles (one persistent CTA per SM, 544 threads):
+//   warp 16      TMA producer: cp.async.bulk.tensor boxes {rows, 8 channels} of the raw fp32 operand tensors -> raw ring
 //                (zero fill outside the tensor = the conv's zero padding of the raw rows; mbarrier complete_tx)
-//   warps 9..16  transform: raw ring -> BN-apply / GELU (forward) or BN-backward / dropout / sigmoid' (data gradient)
+//   warps 8..15  transform: raw ring -> BN-apply / GELU (forward) or BN-backward / dropout / sigmoid' (data gradient)
 //                -> exact hi + lo TF32 split -> panel ring (generic stores + fence.proxy.async)
-//   warp 8       MMA issuer: one elected thread, tcgen05.mma kind::tf32, 3 passes (hi*hi + lo*hi + hi*lo ~ fp32 products),
-//                tcgen05.commit releases panel stages and publishes the accumulator
-//   warps 0..7   epilogue (two groups of 4, one per TMEM accumulator buffer): tcgen05.ld (lane = sample), bias / dropout /
-//                residual views / BatchNorm statistics (forward) or GELU' / BN-backward sums / accumulate (data gradient),
-//                coalesced 128-byte stores; overlaps the MMAs of the next tile.
+//   warps 0..7   two consumer warpgroups: warpgroup h issues one wgmma.m64nNk8 .tf32 per k-step and pass (N = result
+//                channels padded to 32 / 64 / 128, a template parameter) for rows 64h .. 64h+63 of the tile,
+//                3 passes (hi*hi + lo*hi + hi*lo ~ fp32 products), accumulators in registers; then both park them in a
+//                shared staging tile [channel][sample] and run the epilogue (lane = sample): bias / dropout / residual views
+//                / BatchNorm statistics (forward) or GELU' / BN-backward sums / accumulate (data gradient), coalesced
+//                128-byte stores.  The producer and transform warps stage the next tile meanwhile.
 #include <cuda.h>
 #include <cstdlib>
 #include <cstring>
@@ -28,11 +29,13 @@
 
 namespace seist {
 
-constexpr int TCC_EPI_WARPS = 8;      // two groups of 4 (TMEM lane quadrant = warp % 4); group g drains accumulator buffer g
+constexpr int TCC_EPI_WARPS = 8;      // two consumer warpgroups (MMA + epilogue)
 constexpr int TCC_XF_WARPS = 8;
-constexpr int TCC_NT = 32 * (TCC_EPI_WARPS + 1 + TCC_XF_WARPS + 1);
+constexpr int TCC_NT = 32 * (TCC_EPI_WARPS + TCC_XF_WARPS + 1);
 constexpr int TCC_M = 128;
 constexpr int TCC_MAX_STAGES = 8;
+constexpr int TCC_NMAX = 128;         // result channels: 64 accumulator registers per consumer thread
+constexpr int TCC_ACC_PITCH = TCC_M + 4;  // staging tile row pitch (floats): conflict-free fragment stores
 
 struct TccGeom {
   int mode;             // 0 forward, 1 data gradient
@@ -43,8 +46,8 @@ struct TccGeom {
   int src_len, dst_len; // length of the operand rows / of the result rows
   int KC, nchunks;      // reduction channels per chunk (multiple of 8), chunks
   int R, Rbox, Rp;      // panel rows needed (128+k-1), TMA box rows (R rounded to 4), row pitch of the panel (R rounded to 32)
-  int N_pad;            // UMMA N (multiple of 16)
-  int raw_stages, a_stages, b_resident, tmem_cols, passes;
+  int N_pad;            // MMA N (multiple of 16)
+  int raw_stages, a_stages, b_resident;
   int n_raw;            // raw tensors per stage (forward 1; backward: dxd / du / x as present)
   int raw_tensor_bytes; // KC * Rbox * 4
   int a_part;           // bytes of one precision part of a panel stage: (KC/4) * Rp * 16
@@ -54,7 +57,7 @@ struct TccGeom {
   int up, up_S;         // forward only: the operand is the x2 linear up-sampling (F.interpolate, align_corners=False,
                         // models/seist.py:566) of a source of up_S samples; the raw ring then holds SOURCE rows
   // shared-memory carve-up (byte offsets from the 128-aligned base)
-  int off_raw, off_a, off_b, off_tab_k, off_tab_n, off_red, off_bar, smem_bytes;
+  int off_raw, off_a, off_b, off_tab_k, off_tab_n, off_red, off_acc, off_bar, smem_bytes;
 };
 
 struct TccMaps {
@@ -79,23 +82,45 @@ __device__ int g_tcc_err_dev = 0;
 
 __device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// wgmma shared-memory descriptor: start, LBO (K direction), SBO (M / N direction) in 16-byte units; no swizzle
 __device__ __forceinline__ uint64_t tcc_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version (Blackwell); layout_type 0 = no swizzle
   return d;
 }
-__device__ __forceinline__ void tcc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 operands, fp32 accumulators in the m64nNk8 fragment layout (N / 2 per thread)
+template <int N>
+__device__ __forceinline__ void tcc_mma(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accum);
+template <>
+__device__ __forceinline__ void tcc_mma<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-__device__ __forceinline__ void tcc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+template <>
+__device__ __forceinline__ void tcc_mma<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
+}
+template <>
+__device__ __forceinline__ void tcc_mma<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
+}
+template <int R>
+__device__ __forceinline__ void tcc_keep(float (&d)[R]) {      // accumulator registers are not touched across this point
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ void tcc_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -151,14 +176,9 @@ __device__ __forceinline__ int tcc_red_index(int lane) {
   return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
 }
 
-#define TCC_LD16(rr, taddr)                                                                                              \
-  asm volatile(                                                                                                          \
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];" \
-      : "=r"(rr[0]), "=r"(rr[1]), "=r"(rr[2]), "=r"(rr[3]), "=r"(rr[4]), "=r"(rr[5]), "=r"(rr[6]), "=r"(rr[7]),          \
-        "=r"(rr[8]), "=r"(rr[9]), "=r"(rr[10]), "=r"(rr[11]), "=r"(rr[12]), "=r"(rr[13]), "=r"(rr[14]), "=r"(rr[15])     \
-      : "r"(taddr)                                                                                                       \
-      : "memory");                                                                                                       \
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// 16 staged accumulator columns of one sample row
+#define TCC_LD16(rr, col0)                                                                                               \
+  _Pragma("unroll") for (int c_ = 0; c_ < 16; ++c_) rr[c_] = __float_as_uint(acc_s[((col0) + c_) * TCC_ACC_PITCH + srow]);
 
 // first source row staged for a tile whose panel row 0 is up-sampled position p0 (a multiple of 4): the rows needed start at
 // floor((p0 - 1) / 2); TMA boxes must start 16-byte aligned -> rounded down to a multiple of 4
@@ -176,7 +196,8 @@ __device__ __forceinline__ float tcc_wval(const SeistOp& op, int mode, int t, in
 }
 
 // F_GELU: some input view applies GELU (forward transform / backward epilogue); F_ELEM: element dropout
-template <int MODE, bool F_GELU, bool F_ELEM>
+// NB: MMA width (result channels padded to 32, 64 or 128)
+template <int MODE, bool F_GELU, bool F_ELEM, int NB>
 __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant__ SeistOp op, const __grid_constant__ TccGeom g,
                                                            const __grid_constant__ TccMaps maps) {
   extern __shared__ __align__(16) unsigned char tcc_raw[];
@@ -191,12 +212,11 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
   uint64_t* raw_empty = raw_full + TCC_MAX_STAGES;
   uint64_t* a_full = raw_empty + TCC_MAX_STAGES;
   uint64_t* a_empty = a_full + TCC_MAX_STAGES;
-  uint64_t* t_full = a_empty + TCC_MAX_STAGES;
-  uint64_t* t_empty = t_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
-  volatile int* abort_s = reinterpret_cast<volatile int*>(tmem_slot + 1);
+  volatile int* abort_s = reinterpret_cast<volatile int*>(a_empty + TCC_MAX_STAGES);
+  float* acc_s = reinterpret_cast<float*>(base + g.off_acc);                // accumulator staging [N_pad][TCC_ACC_PITCH]
 
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);     // provably warp-uniform: the role branches hold wgmma
   const int Kd = g.Kd, Nd = g.Nd;
   const int Kd_pad = g.nchunks * g.KC;
   const int tiles_per_n = (g.dst_len + TCC_M - 1) / TCC_M;
@@ -275,39 +295,27 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
       tcc_split(w[3], hi.w, lo.w);
       const int off = (t * nq + q) * colpitchB + n * 16;
       *reinterpret_cast<float4*>(b_hi + off) = hi;
-      if (g.passes > 1) *reinterpret_cast<float4*>(b_lo + off) = lo;
+      *reinterpret_cast<float4*>(b_lo + off) = lo;
     }
   };
   if (g.b_resident)
     for (int ch = 0; ch < g.nchunks; ++ch) stage_b(ch, b_s + (size_t)ch * 2 * g.b_part, b_s + (size_t)ch * 2 * g.b_part + g.b_part, tid, TCC_NT);
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(tmem_slot)), "r"((uint32_t)g.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (tid == 32) {
     for (int i = 0; i < TCC_MAX_STAGES; ++i) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&raw_full[i])), "r"(1) : "memory");
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&raw_empty[i])), "r"(TCC_XF_WARPS) : "memory");
       asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&a_full[i])), "r"(TCC_XF_WARPS) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&a_empty[i])), "r"(1) : "memory");
-    }
-    for (int i = 0; i < 2; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&t_full[i])), "r"(1) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&t_empty[i])), "r"(4) : "memory");
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(&a_empty[i])), "r"(TCC_EPI_WARPS) : "memory");
     }
     *abort_s = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // resident weights: generic writes -> async proxy
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   const uint64_t seed = load_seed(op.step_seed);
 
-  if (warp == TCC_EPI_WARPS + 1 + TCC_XF_WARPS) {
+  if (warp == TCC_EPI_WARPS + TCC_XF_WARPS) {
     // =========================== TMA producer ===========================
     if (lane == 0) {
       int rs = 0;
@@ -342,11 +350,11 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
         }
       }
     }
-  } else if (warp > TCC_EPI_WARPS) {
+  } else if (warp >= TCC_EPI_WARPS) {
     // =========================== transform warps ===========================
     // warp -> one channel quad q (its 4 coefficient rows stay in registers for the whole chunk) and every
     // (8 / nq)-th 32-row block of the panel; lane = panel row
-    const int xw = warp - (TCC_EPI_WARPS + 1);
+    const int xw = warp - TCC_EPI_WARPS;
     int rs = 0, as = 0;
     uint32_t rph = 0, aph = 0;
     const int nq = g.KC >> 2, nrb = g.Rp >> 5;
@@ -444,7 +452,7 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
             tcc_split(t[h][2], hi.z, lo.z);
             tcc_split(t[h][3], hi.w, lo.w);
             *reinterpret_cast<float4*>(a_hi + rrow[h] * 16) = hi;
-            if (g.passes > 1) *reinterpret_cast<float4*>(a_lo + rrow[h] * 16) = lo;
+            *reinterpret_cast<float4*>(a_lo + rrow[h] * 16) = lo;
           }
         }
         if (!g.b_resident) {
@@ -461,58 +469,12 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
         if (++as == g.a_stages) { as = 0; aph ^= 1; }
       }
     }
-  } else if (warp == TCC_EPI_WARPS) {
-    // =========================== MMA issuer ===========================
-    int as = 0;
-    uint32_t aph = 0;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(g.N_pad >> 3) << 17) | ((uint32_t)(TCC_M >> 4) << 24);
-    const uint32_t colpitchA = (uint32_t)g.Rp * 16u;
-    const int nq = g.KC >> 2;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total && !*abort_s; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t tph = (uint32_t)(it >> 1) & 1u;
-      if (!tcc_wait(s32(&t_empty[acc]), tph ^ 1, abort_s)) break;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t d_tmem = tmem_base + (uint32_t)(acc * g.N_pad);
-      bool ok = true;
-      for (int ch = 0; ch < g.nchunks; ++ch) {
-        if (!tcc_wait(s32(&a_full[as]), aph, abort_s)) { ok = false; break; }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (lane == 0) {
-          const uint32_t a_hi = s32(a_s + (size_t)as * g.a_stage);
-          const uint32_t a_lo = a_hi + (uint32_t)g.a_part;
-          uint32_t b_hi;
-          if (g.b_resident) b_hi = s32(b_s + (size_t)ch * 2 * g.b_part);
-          else b_hi = a_hi + 2u * (uint32_t)g.a_part;
-          const uint32_t b_lo = b_hi + (uint32_t)g.b_part;
-          const int ksteps = min(g.KC, Kd - ch * g.KC + 7) >> 3;
-          for (int t = 0; t < g.k; ++t) {
-            for (int j = 0; j < ksteps; ++j) {
-              const uint32_t aoff = (uint32_t)(2 * j) * colpitchA + (uint32_t)(t + g.toff) * 16u;
-              const uint32_t boff = (uint32_t)(t * nq + 2 * j) * (uint32_t)colpitchB;
-              const uint64_t ah = tcc_desc(a_hi + aoff, colpitchA, 128);
-              const uint64_t bh = tcc_desc(b_hi + boff, (uint32_t)colpitchB, 128);
-              tcc_mma(d_tmem, ah, bh, idesc, (ch > 0 || t > 0 || j > 0) ? 1u : 0u);
-              if (g.passes > 1) {
-                const uint64_t al = tcc_desc(a_lo + aoff, colpitchA, 128);
-                const uint64_t bl = tcc_desc(b_lo + boff, (uint32_t)colpitchB, 128);
-                tcc_mma(d_tmem, al, bh, idesc, 1u);
-                tcc_mma(d_tmem, ah, bl, idesc, 1u);
-              }
-            }
-          }
-          tcc_commit(s32(&a_empty[as]));
-          if (ch + 1 == g.nchunks) tcc_commit(s32(&t_full[acc]));
-        }
-        __syncwarp();
-        if (++as == g.a_stages) { as = 0; aph ^= 1; }
-      }
-      if (!ok) break;
-    }
   } else {
-    // =========================== epilogue warps ===========================
-    // group eg = warp / 4 drains accumulator buffer eg (tiles it = eg, eg + 2, ...); TMEM lanes 32 * (warp % 4) ..
+    // =========================== consumer warpgroups ===========================
+    // warpgroup eg = warp / 4 multiplies rows 64 eg .. 64 eg + 63 of every tile into registers, both park their
+    // accumulators in acc_s, then run the epilogue of the tile together: group eg takes the 16-channel chunks
+    // c0 / 16 = eg (mod 2), warp % 4 a 32-row quadrant, lane = sample.  The tile loop does not test the abort flag, so
+    // that both groups always meet at the named barriers; after an abort they only skip the work.
     const int eg = warp >> 2, wq = warp & 3;
     const int L = g.dst_len;
     const bool stats = MODE == 0 ? ((op.out.bn >= 0) && op.bn_table[op.out.bn >= 0 ? op.out.bn : 0].use_batch) : true;
@@ -524,25 +486,76 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
     const bool has_ra = MODE == 0 && op.res_a.C > 0, has_rb = MODE == 0 && op.res_b.C > 0;
     const bool sig = op.out_act == SEIST_OUT_SIGMOID;
     const size_t Ls = (size_t)L;
-    int it = eg;
-    for (int tile = blockIdx.x + eg * gridDim.x; tile < total && !*abort_s; tile += 2 * gridDim.x, it += 2) {
-      const uint32_t tph = (uint32_t)(it >> 1) & 1u;
+    const uint32_t colpitchA = (uint32_t)g.Rp * 16u;
+    const int nq = g.KC >> 2;
+    const int srow = 32 * wq + lane;                     // staged sample row this thread reads in the epilogue
+    int as = 0;
+    uint32_t aph = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      float acc[NB / 2];
+      bool run = true;
+      int prev = -1;                                     // stage whose MMAs may still be in flight
+      for (int ch = 0; ch < g.nchunks; ++ch) {
+        // issued whether or not the wait succeeded: a predicated wgmma serialises, and after an abort (bounded wait timed
+        // out) the result of the tile is discarded anyway
+        run = run && tcc_wait(s32(&a_full[as]), aph, abort_s);
+        {
+          const uint32_t a_hi = s32(a_s + (size_t)as * g.a_stage) + (uint32_t)(eg * 64 * 16);
+          const uint32_t a_lo = a_hi + (uint32_t)g.a_part;
+          uint32_t b_hi;
+          if (g.b_resident) b_hi = s32(b_s + (size_t)ch * 2 * g.b_part);
+          else b_hi = s32(a_s + (size_t)as * g.a_stage) + 2u * (uint32_t)g.a_part;
+          const uint32_t b_lo = b_hi + (uint32_t)g.b_part;
+          const int ksteps = min(g.KC, Kd - ch * g.KC + 7) >> 3;
+          asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+          for (int t = 0; t < g.k; ++t) {
+            for (int j = 0; j < ksteps; ++j) {
+              const uint32_t aoff = (uint32_t)(2 * j) * colpitchA + (uint32_t)(t + g.toff) * 16u;
+              const uint32_t boff = (uint32_t)(t * nq + 2 * j) * (uint32_t)colpitchB;
+              const uint64_t ah = tcc_desc(a_hi + aoff, colpitchA, 128), al = tcc_desc(a_lo + aoff, colpitchA, 128);
+              const uint64_t bh = tcc_desc(b_hi + boff, (uint32_t)colpitchB, 128), bl = tcc_desc(b_lo + boff, (uint32_t)colpitchB, 128);
+              tcc_mma<NB>(acc, ah, bh, (ch > 0 || t > 0 || j > 0) ? 1u : 0u);
+              tcc_mma<NB>(acc, al, bh, 1u);
+              tcc_mma<NB>(acc, ah, bl, 1u);
+            }
+          }
+          asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+          asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the previous chunk's MMAs are done
+        }
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) tcc_arrive(s32(&a_empty[prev]));   // this warp's reads of that stage are complete
+        }
+        prev = as;
+        if (++as == g.a_stages) { as = 0; aph ^= 1; }
+      }
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+      tcc_keep(acc);
+      __syncwarp();
+      if (lane == 0) tcc_arrive(s32(&a_empty[prev]));
+      asm volatile("bar.sync 1, 256;" ::: "memory");    // the previous tile's epilogue is done with acc_s
+      if (run) {
+        const int r0 = eg * 64 + wq * 16 + (lane >> 2);
+        const int cl = 2 * (lane & 3);
+#pragma unroll
+        for (int e = 0; e < NB / 2; ++e)
+          acc_s[(8 * (e >> 2) + cl + (e & 1)) * TCC_ACC_PITCH + r0 + 8 * ((e >> 1) & 1)] = acc[e];
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (!run || *abort_s) continue;
       const int n = tile / tiles_per_n;
-      const int l = (tile - n * tiles_per_n) * TCC_M + 32 * wq + lane;
+      const int l = (tile - n * tiles_per_n) * TCC_M + srow;
       const bool ok = l < L;
       const int ls = ok ? l : 0;
-      if (!tcc_wait(s32(&t_full[eg]), tph, abort_s)) break;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t trow = tmem_base + ((uint32_t)(32 * wq) << 16) + (uint32_t)(eg * g.N_pad);
       if (MODE == 0) {
         const float pf = path_factor(op, seed, n), af = alpha_factor(op, seed, n);
-        float* optr = op.out.x + ((size_t)n * op.out.Ct + op.out.c0) * Ls + ls;
-        const float* ra = has_ra ? op.res_a.x + ((size_t)n * op.res_a.Ct + op.res_a.c0) * Ls + ls : nullptr;
-        const float* rb = has_rb ? op.res_b.x + ((size_t)n * op.res_b.Ct + op.res_b.c0) * Ls + ls : nullptr;
+        float* optr = op.out.x + ((size_t)n * op.out.Ct + op.out.c0 + 16 * eg) * Ls + ls;
+        const float* ra = has_ra ? op.res_a.x + ((size_t)n * op.res_a.Ct + op.res_a.c0 + 16 * eg) * Ls + ls : nullptr;
+        const float* rb = has_rb ? op.res_b.x + ((size_t)n * op.res_b.Ct + op.res_b.c0 + 16 * eg) * Ls + ls : nullptr;
 #pragma unroll 1
-        for (int c0 = 0; c0 < Nd; c0 += 16) {
+        for (int c0 = 16 * eg; c0 < Nd; c0 += 32) {
           uint32_t rr[16];
-          TCC_LD16(rr, trow + (uint32_t)c0);
+          TCC_LD16(rr, c0);
           const int nv = min(16, Nd - c0);               // uniform
           float val[16];
 #pragma unroll
@@ -565,7 +578,7 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
             for (int c = 0; c < 16; ++c) rv[c] = __ldg(ra + (size_t)min(c, nv - 1) * Ls);
 #pragma unroll
             for (int c = 0; c < 16; ++c) val[c] += fmaf(ep_s[Nd + min(c0 + c, Nd - 1)], rv[c], ep_s[2 * Nd + min(c0 + c, Nd - 1)]);
-            ra += 16 * Ls;
+            ra += 32 * Ls;
           }
           if (af != 1.f) {
 #pragma unroll
@@ -577,7 +590,7 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
             for (int c = 0; c < 16; ++c) rv[c] = __ldg(rb + (size_t)min(c, nv - 1) * Ls);
 #pragma unroll
             for (int c = 0; c < 16; ++c) val[c] += fmaf(ep_s[3 * Nd + min(c0 + c, Nd - 1)], rv[c], ep_s[4 * Nd + min(c0 + c, Nd - 1)]);
-            rb += 16 * Ls;
+            rb += 32 * Ls;
           }
           if (sig) {
 #pragma unroll
@@ -591,7 +604,7 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
             val[c] = w ? val[c] : 0.f;
             op_c += Ls;
           }
-          optr += 16 * Ls;
+          optr += 32 * Ls;
           if (stats) {
             float s2[16];
 #pragma unroll
@@ -606,9 +619,9 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
         }
       } else {
 #pragma unroll 1
-        for (int c0 = 0; c0 < Nd; c0 += 16) {
+        for (int c0 = 16 * eg; c0 < Nd; c0 += 32) {
           uint32_t rr[16];
-          TCC_LD16(rr, trow + (uint32_t)c0);
+          TCC_LD16(rr, c0);
           float xv[16], ov[16];
 #pragma unroll
           for (int c = 0; c < 16; ++c) {
@@ -638,16 +651,11 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) tcc_arrive(s32(&t_empty[eg]));
     }
   }
 
   // ---- teardown ---------------------------------------------------------------------------------------------------
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
   if (MODE == 0) {
     const bool stats = (op.out.bn >= 0) && op.bn_table[op.out.bn >= 0 ? op.out.bn : 0].use_batch;
     if (stats) {
@@ -669,9 +677,6 @@ __global__ void __launch_bounds__(TCC_NT, 1) tcconv_kernel(const __grid_constant
         atomicAdd(&e.gstat_acc[(i & 1) * e.C + t.bnc], (double)s);
       }
     }
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)g.tmem_cols) : "memory");
   }
   if (tid == 0 && *abort_s) atomicExch(&g_tcc_err_dev, 1);
 }
@@ -711,14 +716,10 @@ static int tcc_make_map(CUtensorMap* m, const float* basep, int L, int Ct, int N
   return 0;
 }
 
-static int tcc_passes() {
-  static int v = -1;
-  if (v < 0) { const char* e = std::getenv("SEIST_TC_PASSES"); v = (e && e[0] == '1') ? 1 : 3; }
-  return v;
-}
 
 bool tcconv_eligible(const SeistOp& op, int mode) {
   if (op.stride != 1 || op.pool > 1 || op.k > 32) return false;
+  if ((mode == 0 ? op.Cout : op.Cin) > TCC_NMAX) return false;   // accumulator registers of the consumer warpgroups
   if (op.L_in != op.L_out || (op.L_out & 3)) return false;       // TMA: 16-byte row pitch
   if (op.up_src_L > 0) {     // x2 linear up-sampling folded into the forward transform (the dpk head, models/seist.py:560-566)
     if (mode != 0 || op.n_in != 1 || op.L_in != 2 * op.up_src_L || (op.up_src_L & 3) || op.in[0].L != op.up_src_L) return false;
@@ -756,11 +757,8 @@ static bool tcc_geometry(const SeistOp& op, int mode, TccGeom& g) {
   g.up_S = op.up_src_L;
   g.Rbox = g.up ? ((g.R / 2 + 6 + 3) & ~3) : ((g.R + 3) & ~3);       // raw rows staged per tile (source rows when up-sampling)
   g.Rp = (g.R + 31) & ~31;
-  g.N_pad = (g.Nd + 15) & ~15;
-  g.passes = tcc_passes();
-  g.tmem_cols = 32;
-  while (g.tmem_cols < 2 * g.N_pad) g.tmem_cols <<= 1;
-  if (g.tmem_cols > 512) return false;
+  g.N_pad = g.Nd <= 32 ? 32 : (g.Nd <= 64 ? 64 : 128);
+  if (g.N_pad > TCC_NMAX) return false;
   const bool has_bn = (op.out.bn >= 0 && op.out.g != nullptr);
   g.has_dxd = (mode == 1 && op.out_dxd != nullptr) ? 1 : 0;
   g.has_bn = (mode == 1 && has_bn) ? 1 : 0;
@@ -791,7 +789,8 @@ static bool tcc_geometry(const SeistOp& op, int mode, TccGeom& g) {
       const int a_stage = 2 * g.a_part + (resident ? 0 : 2 * g.b_part);
       g.a_stage = a_stage;
       const int raw_stage = g.n_raw * g.raw_tensor_bytes;
-      const int fixed = b_bytes + g.nchunks * KC * (int)sizeof(TccK) + tab_n + 16 * g.Nd * 4 + (4 * TCC_MAX_STAGES + 4) * 8 + 64 + 256;
+      const int acc_bytes = g.N_pad * TCC_ACC_PITCH * 4;
+      const int fixed = b_bytes + g.nchunks * KC * (int)sizeof(TccK) + tab_n + 16 * g.Nd * 4 + acc_bytes + 4 * TCC_MAX_STAGES * 8 + 64 + 256;
       for (int st = 4; st >= 2; --st) {
         const int rst = st + 1 > TCC_MAX_STAGES ? TCC_MAX_STAGES : st + 1;
         const int tot = fixed + st * a_stage + rst * raw_stage;
@@ -808,7 +807,8 @@ static bool tcc_geometry(const SeistOp& op, int mode, TccGeom& g) {
           off = (off + 15) & ~15;
           g.off_red = off; off += 16 * g.Nd * 4;
           off = (off + 15) & ~15;
-          g.off_bar = off; off += (4 * TCC_MAX_STAGES + 4) * 8 + 64;
+          g.off_acc = off; off += acc_bytes;
+          g.off_bar = off; off += 4 * TCC_MAX_STAGES * 8 + 64;
           g.smem_bytes = off + 128;
           return true;
         }
@@ -818,18 +818,24 @@ static bool tcc_geometry(const SeistOp& op, int mode, TccGeom& g) {
   return false;
 }
 
-template <int MODE, bool G, bool E>
-static int tcc_go(const SeistOp& op, const TccGeom& g, const TccMaps& maps, unsigned grid, cudaStream_t s) {
+template <int MODE, bool G, bool E, int NB>
+static int tcc_go_nb(const SeistOp& op, const TccGeom& g, const TccMaps& maps, unsigned grid, cudaStream_t s) {
   static bool attr_set[64] = {false};        // the attribute is per device
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_set[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(tcconv_kernel<MODE, G, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(tcconv_kernel<MODE, G, E, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return (int)e; }
     attr_set[dev & 63] = true;
   }
-  tcconv_kernel<MODE, G, E><<<grid, TCC_NT, g.smem_bytes, s>>>(op, g, maps);
+  tcconv_kernel<MODE, G, E, NB><<<grid, TCC_NT, g.smem_bytes, s>>>(op, g, maps);
   return 0;
+}
+template <int MODE, bool G, bool E>
+static int tcc_go(const SeistOp& op, const TccGeom& g, const TccMaps& maps, unsigned grid, cudaStream_t s) {
+  if (g.N_pad == 32) return tcc_go_nb<MODE, G, E, 32>(op, g, maps, grid, s);
+  if (g.N_pad == 64) return tcc_go_nb<MODE, G, E, 64>(op, g, maps, grid, s);
+  return tcc_go_nb<MODE, G, E, 128>(op, g, maps, grid, s);
 }
 
 int launch_tcconv(const SeistOp& op, int mode, cudaStream_t s, int sm_count) {

@@ -1,6 +1,6 @@
 """Model registry and checkpoint I/O with the reference's contract.
 
-Mirrors /root/reference/models/_factory.py: `register_model` (:24-38) keys the registry by the
+Mirrors the reference's models/_factory.py: `register_model` (:24-38) keys the registry by the
 creator's ``__name__`` and rejects duplicates; `create_model` (:41-56) raises ValueError listing
 what is available; `save_checkpoint` (:59-87) / `load_checkpoint` (:90-126) keep the reference's
 checkpoint dictionary layout so files are interchangeable in both directions.

@@ -1,7 +1,7 @@
 """SeisT (Seismogram Transformer) behind the reference's `@register_model` surface, executed by
-hand-written sm_100a CUDA kernels.
+hand-written sm_90a CUDA kernels.
 
-What is kept from the reference (/root/reference/models/seist.py): the registered creator names
+What is kept from the reference (models/seist.py): the registered creator names
 (:940-1170), the hyper-parameter presets (:855-937), and the *parameter tree* — every
 nn.Conv1d / nn.BatchNorm1d / nn.Linear lives at the same attribute path, so `state_dict()` keys,
 shapes and dtypes are identical (SURVEY §3.4) and the reference's `pretrained/*.pth` load with
@@ -296,7 +296,7 @@ class SeismogramTransformer(nn.Module):
         # `torch.compile(model)` (the reference's default, training/train.py:296-297) degrades to a graph break here:
         # the forward is one opaque call into the C-ABI plan executor, there is nothing for Inductor to fuse
         if not x.is_cuda:
-            raise RuntimeError("seist_b200 has no CPU path: the input must live on a CUDA (sm_100a) device")
+            raise RuntimeError("seist_b200 has no CPU path: the input must live on a CUDA (sm_90a) device")
         return self.engine().forward(x)
 
     def _apply(self, fn, *args, **kwargs):

@@ -9,7 +9,7 @@ consuming kernel evaluates while loading, or as an epilogue of the producing ker
 plan is derived here from the forward tape: each forward op emits up to three backward ops, and the
 compiler tracks which gradient buffers have been written to choose overwrite vs accumulate.
 
-Reference semantics cited per emitter (paths relative to /root/reference/models/seist.py).
+Reference semantics cited per emitter (paths relative to the reference's models/seist.py).
 """
 from __future__ import annotations
 
@@ -224,9 +224,8 @@ class PlanBuilder:
         self.mods = dict(model.named_modules())
         self.seed_ctr = 1
         # SEIST_BN_INLINE=1 (single-GPU training): no BN_PREPARE launches (216 per seist_m_dpk step), every consumer CTA
-        # derives the per-channel coefficients from the statistics while it resolves its views.  Measured on B200: 596
-        # instead of 812 launches but 43.2 instead of 41.1 ms/step - the fp64 divisions / rsqrt repeated by every CTA cost
-        # more than the launches they save (gpurun_out/bench_r2h.json) - so the separate launches stay the default.
+        # derives the per-channel coefficients from the statistics while it resolves its views.  The fp64 divisions / rsqrt
+        # repeated by every CTA cost more than the launches they save, so the separate launches stay the default.
         self.inline_coef = bool(training and world == 1 and os.environ.get("SEIST_BN_INLINE", "0") == "1")
         self._bn_idx: Dict[str, int] = {}
         self._st_off = 0
@@ -562,9 +561,8 @@ class PlanBuilder:
     def _wants_combine(f: Op) -> bool:
         """Evaluate the BN backward of f's output once (GRAD_COMBINE) instead of in every pass of its three
         backward ops?  Pays off when the data gradient needs several 16-channel passes over the output gradient
-        (wide 1x1 convs): each pass then loads one tensor instead of (du, x[, dxd]).  Measured on B200 it is a wash
-        (the combine passes cost what the backward ops save, profiles/), so it is OFF by default; SEIST_COMBINE_CIN=<min
-        reduction width> enables it."""
+        (wide 1x1 convs): each pass then loads one tensor instead of (du, x[, dxd]).  The combine passes cost about
+        what the backward ops save, so it is OFF by default; SEIST_COMBINE_CIN=<min reduction width> enables it."""
         thr = int(os.environ.get("SEIST_COMBINE_CIN", "0"))
         if thr <= 0 or f.out is None or f.out.bn < 0 or not f.out.buf.need_du:
             return False

@@ -182,7 +182,7 @@ def _cost(op) -> float:
 
 
 def n_main_lanes() -> int:
-    """main lanes (critical chain + independent branches); SEIST_NMAIN=1..3, default 2 (measured: profiles/r2_knob_sweeps.txt)"""
+    """main lanes (critical chain + independent branches); SEIST_NMAIN=1..3, default 2"""
     return min(3, max(1, int(os.environ.get("SEIST_NMAIN", "2"))))
 
 

@@ -6,6 +6,7 @@ import os
 import pytest
 import torch
 
+from oracle import golden as G
 from oracle import seist_ref as R
 from oracle.plan_interp import Interp, keep_mask, rng_u16
 from seist_b200 import _lib
@@ -14,7 +15,6 @@ from seist_b200 import models
 from seist_b200.models import create_model, get_model_list, register_model
 from seist_b200.models.seist import dpk_up_sizes, same_pad, split_mptl, split_msmc
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ZERO = dict(path_drop_rate=0, attn_drop_rate=0, key_drop_rate=0, mlp_drop_rate=0, other_drop_rate=0)
 
 
@@ -34,13 +34,11 @@ def test_registry_surface():
 
 @pytest.mark.parametrize("name", ["seist_s_dpk", "seist_m_dpk", "seist_m_emg"])
 def test_state_dict_matches_reference_checkpoint(name):
-    g = torch.load(os.path.join(GOLD, f"{name}.pt"))
+    g = G.load(name)
     m = create_model(name, in_channels=3, in_samples=8192)
-    sd = m.state_dict()
-    assert list(sd.keys()) == list(g["state_dict"].keys())
-    for k, v in g["state_dict"].items():
-        assert sd[k].shape == v.shape and sd[k].dtype == v.dtype, k
+    assert G.digest(G.layout(m.state_dict())) == g["layout_sha"]          # keys, shapes and dtypes, in order
     m.load_state_dict(g["state_dict"], strict=True)
+    assert G.digest([k for k, _ in m.named_parameters()]) == g["param_sha"]
     assert [k for k, _ in m.named_parameters()] == list(g["grads"].keys())
 
 
@@ -67,7 +65,7 @@ def test_channel_arithmetic():
 def test_plan_compiler_end_to_end_vs_reference_golden():
     """Forward tape, derived backward, accumulate flags and the BN-backward algebra, executed by the CPU
     interpreter, reproduce the reference's outputs, gradients and running statistics."""
-    g = torch.load(os.path.join(GOLD, "seist_s_dpk.pt"))
+    g = G.load("seist_s_dpk")
     m = create_model("seist_s_dpk", in_channels=3, in_samples=8192)
     m.load_state_dict(g["state_dict"], strict=True)
     m.set_drop_rates(**ZERO)
@@ -76,29 +74,29 @@ def test_plan_compiler_end_to_end_vs_reference_golden():
     pl = P.PlanBuilder(m, flat, 2, 8192, training=False).build()
     P.allocate(pl, False)
     y = Interp(pl).run_fwd(x)
-    assert (y - g["y_eval"][:2]).abs().max().item() < 1e-4
+    assert g["y_eval"].err(y) < 1e-4          # the first two waveforms of the fixture
     # train mode on the full fixture batch (statistics depend on the batch)
     x = g["x"]
     pl = P.PlanBuilder(m, flat, x.shape[0], 8192, training=True).build()
     P.allocate(pl, True)
     it = Interp(pl)
     y = it.run_fwd(x).clone()
-    assert (y - g["y_train"]).abs().max().item() < 1e-4
+    assert g["y_train"].err(y) < 1e-4
     p = y.clone().requires_grad_(True)
     R.bce_loss(p, g["target"]).backward()
     it.run_bwd(p.grad)
-    gmax = max(v.abs().max().item() for v in g["grads"].values())
+    gmax = max(v.absmax for v in g["grads"].values())
     for k, ref in g["grads"].items():
-        err = (flat.grad_view(k) - ref).abs().max().item()
-        assert err <= 1e-3 * ref.abs().max().item() + 1e-6 * gmax, (k, err)
+        err = ref.err(flat.grad_view(k))
+        assert err <= 1e-3 * ref.absmax + 1e-6 * gmax, (k, err)
     sd = m.state_dict()
     for k, b in g["buffers_after"].items():
-        assert (sd[k].float() - b.float()).abs().max().item() <= 1e-3 * (b.float().abs().max().item() + 1e-3), k
+        assert b.err(sd[k].float()) <= 1e-3 * (b.absmax + 1e-3), k
 
 
 def test_plan_compiler_regression_head_vs_reference_golden():
     """Same as above for the regression family (seist_m_emg: HEADVEC ops, scaled sigmoid, Huber loss)."""
-    g = torch.load(os.path.join(GOLD, "seist_m_emg.pt"))
+    g = G.load("seist_m_emg")
     m = create_model("seist_m_emg", in_channels=3, in_samples=8192)
     m.load_state_dict(g["state_dict"], strict=True)
     m.set_drop_rates(**ZERO)
@@ -108,20 +106,20 @@ def test_plan_compiler_regression_head_vs_reference_golden():
     P.allocate(pl, False)
     y = Interp(pl).run_fwd(x)
     y = y if y.dim() == 2 else y[:, :, 0]
-    assert (y - g["y_eval"]).abs().max().item() < 1e-4 * max(1.0, g["y_eval"].abs().max().item())
+    assert g["y_eval"].err(y) < 1e-4 * max(1.0, g["y_eval"].absmax)
     pl = P.PlanBuilder(m, flat, x.shape[0], 8192, training=True).build()
     P.allocate(pl, True)
     it = Interp(pl)
     y = it.run_fwd(x).clone()
     y2 = y if y.dim() == 2 else y[:, :, 0]
-    assert (y2 - g["y_train"]).abs().max().item() < 1e-4 * max(1.0, g["y_train"].abs().max().item())
+    assert g["y_train"].err(y2) < 1e-4 * max(1.0, g["y_train"].absmax)
     p = y2.clone().requires_grad_(True)
     R.huber_loss(p, g["target"]).backward()
     it.run_bwd(p.grad.reshape(y.shape))
-    gmax = max(v.abs().max().item() for v in g["grads"].values())
+    gmax = max(v.absmax for v in g["grads"].values())
     for k, ref in g["grads"].items():
-        err = (flat.grad_view(k) - ref).abs().max().item()
-        assert err <= 1e-3 * ref.abs().max().item() + 1e-6 * gmax, (k, err)
+        err = ref.err(flat.grad_view(k))
+        assert err <= 1e-3 * ref.absmax + 1e-6 * gmax, (k, err)
 
 
 ALL_VARIANTS = [f"seist_{size}_{task}" for size in "sml" for task in ("dpk", "pmp", "emg", "baz", "dis")]
@@ -162,7 +160,7 @@ def test_grad_combine_plan_equals_default_plan(monkeypatch):
     """GRAD_COMBINE (opt-in, SEIST_COMBINE_CIN): the compiler marks the wide 1x1 convs, emits the in-place BN
     backward before their three backward ops and re-points those ops at the combined gradient; executed by the
     interpreter the parameter gradients must equal the default plan's (reference golden batch, train mode)."""
-    g = torch.load(os.path.join(GOLD, "seist_s_dpk.pt"))
+    g = G.load("seist_s_dpk")
     x = g["x"][:2, :, :2048].contiguous()
     tgt = g["target"][:2, :, :2048].contiguous()
 

@@ -1,23 +1,32 @@
-"""not-gpu: the oracle restatement against the golden vectors produced by the unmodified reference, and
-(in the build container, where /root/reference exists) against the reference's own modules."""
+"""not-gpu: the oracle restatement against the golden vectors produced by the unmodified reference
+(tests/golden/make_golden.py): the model fixtures, train-mode outputs of more variants and the dropout sites of the
+reference's own modules."""
 import os
 
 import pytest
 import torch
 
-from oracle import reference_import as ri
+from oracle import golden as G
 from oracle import seist_ref as R
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+MODULE_MODELS = ("seist_s_dpk", "seist_l_emg", "seist_s_pmp")
+MODULE_L, MODULE_SEED = 2048, G.PARAM_SEED + 1
+SITE_MODELS = ("seist_s_dpk", "seist_m_dpk", "seist_l_dpk", "seist_m_emg")
+
+
+def module_input():
+    return torch.randn(2, 3, MODULE_L, generator=torch.Generator().manual_seed(3))
 
 
 @pytest.mark.parametrize("name", ["seist_s_dpk", "seist_m_dpk", "seist_m_emg", "seist_s_pmp", "seist_s_baz"])
 def test_oracle_matches_golden(name):
-    g = torch.load(os.path.join(GOLD, f"{name}.pt"))
+    g = G.load(name)
     spec = R.spec_for(name)
     with torch.no_grad():
         y, _ = R.forward(g["state_dict"], g["x"], spec, training=False)
-    assert (y - g["y_eval"]).abs().max().item() <= 2e-5 * g["y_eval"].abs().max().item()
+    assert tuple(y.shape) == g["y_eval"].shape
+    assert g["y_eval"].err(y) <= 2e-5 * g["y_eval"].absmax
     if name != "seist_s_dpk":
         return      # one full backward on CPU is enough for the time budget
     sd = {k: (v.clone().requires_grad_(True) if v.dtype.is_floating_point and "running" not in k else v)
@@ -26,27 +35,20 @@ def test_oracle_matches_golden(name):
     loss = R.bce_loss(y, g["target"])
     loss.backward()
     assert abs(loss.item() - g["loss"].item()) <= 1e-5 * abs(g["loss"].item())
-    gmax = max(v.abs().max().item() for v in g["grads"].values())
+    gmax = max(v.absmax for v in g["grads"].values())
     for k, ref in g["grads"].items():
-        assert (sd[k].grad - ref).abs().max().item() <= 1e-4 * ref.abs().max().item() + 1e-6 * gmax, k
+        assert ref.err(sd[k].grad) <= 1e-4 * ref.absmax + 1e-6 * gmax, k
     for k, b in g["buffers_after"].items():
-        assert (bufs[k].float() - b.float()).abs().max().item() <= 1e-5 * (b.float().abs().max().item() + 1e-3), k
+        assert b.err(bufs[k].float()) <= 1e-5 * (b.absmax + 1e-3), k
 
 
-@pytest.mark.skipif(not ri.available(), reason="reference checkout not present (GPU box)")
 def test_oracle_matches_reference_modules():
-    M = ri.import_reference_models()
-    torch.manual_seed(0)
-    for name in ("seist_s_dpk", "seist_l_emg", "seist_s_pmp"):
-        ref = ri.zero_drop_rates(M.create_model(name, in_channels=3, in_samples=2048))
-        with torch.no_grad():   # de-generate the init a little so the comparison is meaningful
-            for p in ref.parameters():
-                p.add_(0.05 * torch.randn_like(p))
-        x = torch.randn(2, 3, 2048)
-        ref.train()
-        y_ref = ref(x)
-        y, _ = R.forward(ref.state_dict(), x, R.spec_for(name), training=True)
-        assert torch.allclose(y, y_ref, atol=1e-6), name
+    ref = torch.load(os.path.join(GOLD, "reference_functions.pt"))["modules"]
+    for name in MODULE_MODELS:
+        sd = G.model_state_dict(name, MODULE_L, seed=MODULE_SEED)
+        y, _ = R.forward(sd, module_input(), R.spec_for(name), training=True)
+        s = G.unpack(ref[name], [tuple(y.shape)])[0]
+        assert torch.allclose(y.detach().reshape(-1)[s.idx], s.val, atol=1e-6), name
 
 
 def test_pad_and_sizes():
@@ -65,8 +67,7 @@ def test_pad_and_sizes():
                                                          (16, 16, 7), (16, 6, 11)]
 
 
-@pytest.mark.skipif(not ri.available(), reason="reference checkout not present (GPU box)")
-@pytest.mark.parametrize("name", ["seist_s_dpk", "seist_m_dpk", "seist_l_dpk", "seist_m_emg"])
+@pytest.mark.parametrize("name", SITE_MODELS)
 def test_dropout_sites_and_rates_match_reference_modules(name):
     """Every nn.Dropout / timm DropPath of the unmodified reference model (site = module path, rate = .p / .drop_prob,
     models/seist.py:114,228,239,360-366,446,470,484; linspace schedule :705) must appear in the compiled plan as the
@@ -74,17 +75,8 @@ def test_dropout_sites_and_rates_match_reference_modules(name):
     from seist_b200 import _lib
     from seist_b200 import plan as P
     from seist_b200.models import create_model
-    M = ri.import_reference_models()
-    ref = M.create_model(name, in_channels=3, in_samples=1024)
     expect = {}
-    for path, mod in ref.named_modules():
-        cls = mod.__class__.__name__
-        if cls == "Dropout":
-            p = float(mod.p)
-        elif cls == "DropPath":
-            p = float(mod.drop_prob or 0.0)
-        else:
-            continue
+    for path, p in torch.load(os.path.join(GOLD, "reference_functions.pt"))["dropout_sites"][name]:
         head, leaf = path.rsplit(".", 1)
         site = {
             "droppath0": (head + ".proj", "p_path"),

@@ -1,22 +1,17 @@
-"""not-gpu: the post-processing oracle (oracle/postprocess_ref.py) against the reference's own `_detect_peaks`, executed
-from its source (the module itself needs obspy / pandas, which are absent; the function only needs numpy)."""
-import ast
+"""not-gpu: the post-processing oracle (oracle/postprocess_ref.py) against what the reference's own `_detect_peaks`
+(training/postprocess.py) returned for the same traces (tests/golden/reference_functions.pt, written by
+tests/golden/make_golden.py)."""
 import os
 
 import numpy as np
 import pytest
+import torch
 
 from oracle import postprocess_ref as PR
-from oracle import reference_import as ri
 
-
-def _reference_detect_peaks():
-    path = os.path.join(ri.REF_ROOT, "training", "postprocess.py")
-    tree = ast.parse(open(path).read())
-    fn = next(n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name == "_detect_peaks")
-    ns = {"np": np}
-    exec(compile(ast.Module(body=[fn], type_ignores=[]), path, "exec"), ns)      # noqa: S102 - the reference's own code
-    return ns["_detect_peaks"]
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_functions.pt")
+CASES = [(1, 50), (3, 50), (5, 8), (2, 200)]
+THRESHOLDS = (0.3, 0.05)
 
 
 def _traces(rng, n, L):
@@ -32,22 +27,25 @@ def _traces(rng, n, L):
     return out
 
 
-@pytest.mark.skipif(not ri.available(), reason="reference checkout not present (GPU box)")
-@pytest.mark.parametrize("topk,mpd", [(1, 50), (3, 50), (5, 8), (2, 200)])
-def test_pick_phase_matches_reference_detect_peaks(topk, mpd):
-    ref = _reference_detect_peaks()
-    rng = np.random.default_rng(topk * 100 + mpd)
-    x = _traces(rng, 48, 2048)
+def peak_traces(topk, mpd):
+    x = _traces(np.random.default_rng(topk * 100 + mpd), 48, 2048)
     x[0] = 0.0                          # no peak at all
     x[1, :] = 0.5                       # flat above the threshold: no rising edge
     x[2] = 0.0
     x[2, 100:110] = 0.8                 # flat-topped peak: rising edge only
     x[3] = 0.0
     x[3, 0], x[3, -1] = 0.9, 0.9        # first / last samples cannot be peaks
-    for thr in (0.3, 0.05):
+    return x
+
+
+@pytest.mark.parametrize("topk,mpd", CASES)
+def test_pick_phase_matches_reference_detect_peaks(topk, mpd):
+    ref = torch.load(GOLD)["detect_peaks"]
+    x = peak_traces(topk, mpd)
+    for thr in THRESHOLDS:
         mine = PR.pick_phase(x, thr, mpd, topk)
-        for i, row in enumerate(x):
-            want = ref(row, mph=thr, mpd=mpd, topk=topk)
+        for i in range(x.shape[0]):
+            want = np.array(ref[(topk, mpd, thr)][i], dtype=np.int64)
             got = mine[i][mine[i] != PR.PAD_PHASE]
             assert np.array_equal(got, want), (i, thr, got, want)
             assert (mine[i][got.size:] == PR.PAD_PHASE).all()

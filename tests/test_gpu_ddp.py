@@ -60,7 +60,7 @@ def test_two_gpu_step_equals_single_gpu_on_concatenated_batch(use_graph, symm):
     memory (comm.cu) - eagerly and as ONE captured CUDA graph per rank (two steps: capture + replay; the first step is
     compared); nccl-fallback: SEIST_SYMM=0, NCCL calls at the plan's sync points."""
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         port = s.getsockname()[1]

@@ -116,7 +116,7 @@ def _run_cases_in_child(env_extra, cases):
     env = dict(os.environ, **env_extra)
     calls = "".join(f"T.test_ops_match_interpreter({c});" for c in cases)
     code = ("import sys; sys.path.insert(0, 'tests'); import test_gpu_ops as T; from seist_b200 import _lib;" + calls +
-            "assert _lib.lib().seist_tc_error_flag() == 0, 'tcgen05 mbarrier wait timed out'; print('TC-OK')")
+            "assert _lib.lib().seist_tc_error_flag() == 0, 'tensor-core mbarrier wait timed out'; print('TC-OK')")
     r = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0 and "TC-OK" in r.stdout, (r.stdout[-2000:], r.stderr[-4000:])
 
@@ -126,22 +126,12 @@ _DROPS = "dict(path_drop_rate=0.3, attn_drop_rate=0.2, key_drop_rate=0.2, mlp_dr
 
 @pytest.mark.gpu
 def test_tcconv_engine_on_every_eligible_op():
-    """The warp-specialised tcgen05 + TMA engine (tcconv.cu) is dispatched by a measured rule (api.cu::tcc_auto); here it
-    is FORCED onto every eligible forward / data-gradient conv (SEIST_TCC=1, read once per process -> child process):
+    """The warp-specialised wgmma + TMA engine (tcconv.cu) is dispatched by a measured rule (api.cu::tcc_auto); here
+    it is FORCED onto every eligible forward / data-gradient conv (SEIST_TCC=1, read once per process -> child process):
     stride-1 k-tap and 1x1 convs of every width, grouped convs, multi-view inputs, residuals, dropout, sigmoid head."""
     _run_cases_in_child({"SEIST_TCC": "1"}, [
         "'seist_m_dpk', 2, 2048, True, None",
         "'seist_l_dpk', 2, 1024, True, None",
         f"'seist_s_dpk', 2, 1024, True, {_DROPS}",
         "'seist_s_dpk', 2, 1024, False, None",
-    ])
-
-
-@pytest.mark.gpu
-def test_legacy_tcgen05_kernels_match_interpreter():
-    """Round-1 tcgen05 kernels (pw_tc forward, bww_tc weight gradient) forced everywhere (SEIST_TC=1) with the new engine
-    off, so that they - not tcconv - serve the 1x1 convs."""
-    _run_cases_in_child({"SEIST_TC": "1", "SEIST_TCC": "0"}, [
-        "'seist_m_dpk', 2, 2048, True, None",
-        f"'seist_s_dpk', 2, 1024, True, {_DROPS}",
     ])
