@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 9
+#define SEIST_ABI_VERSION 10
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -57,8 +57,6 @@ typedef struct SeistBN {
   float eps;
   float momentum;
   float grad_scale;      /* multiplies dgamma/dbeta (1/world_size under data parallelism)         */
-  int32_t inline_coef;   /* 1: consumers derive the coefficients from stat / gstat themselves while resolving their views
-                            (no BN_PREPARE launches: single-GPU training); 0: read the `coef` table           */
 } SeistBN;
 
 /* ---- data-parallel exchange over NVLink peer memory (replaces the per-BatchNorm NCCL calls of
@@ -125,13 +123,7 @@ enum SeistOpKind {
      (out.x) from in[0].x = in_proj [C,C], in[1].x = dconv [C,k], in[2].x = pconv [Cout,C];
      COMPOSE_BWD scatters dW_eff (out.g) into in[0..2].g. */
   SEIST_OP_STEM_COMPOSE_FWD = 15,
-  SEIST_OP_STEM_COMPOSE_BWD = 16,
-  /* BatchNorm backward (the dx of nn.BatchNorm1d the reference's autograd computes, models/seist.py: every
-     *.norm) evaluated ONCE, in place: out.g[n,c,l] <- A*out.g + Bx*out.x + Cc (+ out_dxd) for the channel
-     slice of `out`.  The RES_BWD / CONV_BWD_W / CONV_BWD_DATA ops of the same forward op that follow are then
-     issued with out.bn = -1 and out_dxd = that buffer (a plain gradient: one load instead of three and no
-     prologue arithmetic in each of their passes).  Emitted by the plan compiler for wide 1x1 convolutions. */
-  SEIST_OP_GRAD_COMBINE = 17
+  SEIST_OP_STEM_COMPOSE_BWD = 16
 };
 
 typedef struct SeistOp {

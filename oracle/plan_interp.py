@@ -292,11 +292,9 @@ class Interp:
         p.flat.NBT[:len(p.bns)] += 1
 
     # ---- backward ---------------------------------------------------------------------------------
-    def out_grad(self, f: Op, raw: bool = False) -> torch.Tensor:
+    def out_grad(self, f: Op) -> torch.Tensor:
         o = f.out
         sl = slice(o.c0, o.c0 + o.C)
-        if f.combined and not raw:        # GRAD_COMBINE already left the combined gradient in du
-            return o.buf.du[:, sl].to(self.dt).clone()
         g = torch.zeros(f.N, o.C, o.buf.L, dtype=self.dt)
         if o.buf.dxd is not None:
             g = g + o.buf.dxd[:, sl].to(self.dt)
@@ -339,10 +337,6 @@ class Interp:
             gi, gd, gp = torch.autograd.grad(we, [i, d, pc], dwe)
             for r, gq in zip(f.wparts, (gi, gd, gp)):
                 G[r.off:r.off + r.numel] += gq.reshape(-1).float()
-            return
-        if op.kind == _lib.GRAD_COMBINE:
-            o = f.out
-            o.buf.du[:, o.c0:o.c0 + o.C] = self.out_grad(f, raw=True).float()
             return
         if op.kind == _lib.ZERO:
             (op.out.buf.du if op.out.bn >= 0 else op.out.buf.dxd).zero_()

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 9
+ABI_VERSION = 10
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -22,7 +22,7 @@ class SeistBN(C.Structure):
         ("dgamma", C.c_void_p), ("dbeta", C.c_void_p), ("coef", C.c_void_p),
         ("count", C.c_double),
         ("C", C.c_int32), ("chain", C.c_int32), ("use_batch", C.c_int32), ("is_chained", C.c_int32),
-        ("eps", C.c_float), ("momentum", C.c_float), ("grad_scale", C.c_float), ("inline_coef", C.c_int32),
+        ("eps", C.c_float), ("momentum", C.c_float), ("grad_scale", C.c_float),
     ]
 
 
@@ -72,7 +72,6 @@ HEADVEC_FWD, HEADVEC_BWD = 8, 9
 BN_FINALIZE_FWD, BN_FINALIZE_BWD, ZERO = 10, 11, 12
 BN_PREPARE_FWD, BN_PREPARE_BWD = 13, 14
 STEM_COMPOSE_FWD, STEM_COMPOSE_BWD = 15, 16
-GRAD_COMBINE = 17
 
 _lib = None
 

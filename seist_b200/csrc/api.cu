@@ -45,7 +45,6 @@ bool bww_eligible(const SeistOp& op);
 int launch_bww_any(const SeistOp& op, cudaStream_t s, int sm_count);
 bool convk_eligible(const SeistOp& op);
 bool bwwk_eligible(const SeistOp& op);
-int launch_grad_combine(const SeistOp& op, cudaStream_t s, int sm_count);
 bool convk_bwd_data_eligible(const SeistOp& op);
 int launch_bwwk(const SeistOp& op, cudaStream_t s, int sm_count);
 int launch_convk_fwd(const SeistOp& op, cudaStream_t s);
@@ -56,22 +55,6 @@ bool tcconv_eligible(const SeistOp& op, int mode);
 int launch_tcconv(const SeistOp& op, int mode, cudaStream_t s, int sm_count);
 int tcconv_error_flag();
 
-// integer tuning knob, read from the environment on every call (launch time only; graphs replay the captured choice)
-int env_knob(const char* name, int def) {
-  const char* e = std::getenv(name);
-  return (e && *e) ? std::atoi(e) : def;
-}
-int bww_waves() {
-  static int v = -1;
-  if (v < 0) { const char* e = std::getenv("SEIST_BWW_WAVES"); v = (e && e[0] >= '1' && e[0] <= '4') ? e[0] - '0' : 2; }
-  return v;
-}
-// sliding-window weight-gradient kernel for k > 1 (bwwk.cu); SEIST_BWWK=0 falls back to the row-tiled kernel (A/B runs)
-static int bwwk_mode() {
-  static int v = -1;
-  if (v < 0) { const char* e = std::getenv("SEIST_BWWK"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v;
-}
 // Tensor-core convolution engine (tcconv.cu: wgmma + TMA, 3 x TF32) for stride-1 forward / data-gradient convs.  Measured
 // op by op on H100 at the bench configuration (seist_m_dpk, B = 512, engine forced vs SIMT kernels): it wins on the
 // up-sampled head convs with >= 32 input channels, the k-tap convs of encoder stages 1-3 (forward at L <= 512 with >= 16
@@ -120,13 +103,13 @@ enum Family {
   F_NONE = 0, F_TCCONV_FWD, F_TCCONV_BWD_DATA, F_PW_FWD, F_CONVK_FWD, F_CONV_FWD, F_PW_BWD_DATA, F_CONVK_BWD_DATA,
   F_CONV_BWD_DATA, F_BWWK, F_BWW, F_CONV_BWD_W, F_RES_BWD, F_RES_BWD4, F_ATT_FWD, F_ATT_BWD_Q, F_ATT_BWD_KV, F_HEADVEC_FWD,
   F_HEADVEC_BWD, F_BN_FINALIZE_FWD, F_BN_FINALIZE_BWD, F_BN_PREPARE_FWD, F_BN_PREPARE_BWD, F_STEM_COMPOSE_FWD, F_STEM_COMPOSE_BWD,
-  F_GRAD_COMBINE, F_ZERO
+  F_ZERO
 };
 static const char* kFamilyName[] = {
   "none", "tcconv_fwd(wgmma+TMA)", "tcconv_bwd_data(wgmma+TMA)", "pw_fwd(simt)", "convk_fwd(simt)",
   "conv_fwd(simt)", "pw_bwd_data(simt)", "convk_bwd_data(simt)", "conv_bwd_data(simt)", "bwwk(simt)", "bww(simt)",
   "conv_bwd_w(simt)", "res_bwd", "res_bwd4", "att_fwd", "att_bwd_q", "att_bwd_kv", "headvec_fwd", "headvec_bwd", "bn_finalize_fwd",
-  "bn_finalize_bwd", "bn_prepare_fwd", "bn_prepare_bwd", "stem_compose_fwd", "stem_compose_bwd", "grad_combine", "zero"
+  "bn_finalize_bwd", "bn_prepare_fwd", "bn_prepare_bwd", "stem_compose_fwd", "stem_compose_bwd", "zero"
 };
 
 static Family choose(const SeistOp& op) {
@@ -140,7 +123,7 @@ static Family choose(const SeistOp& op) {
       if (pw_eligible(op)) return F_PW_BWD_DATA;
       return convk_bwd_data_eligible(op) ? F_CONVK_BWD_DATA : F_CONV_BWD_DATA;
     case SEIST_OP_CONV_BWD_W:
-      if (bwwk_mode() && bwwk_eligible(op)) return F_BWWK;
+      if (bwwk_eligible(op)) return F_BWWK;
       return bww_eligible(op) ? F_BWW : F_CONV_BWD_W;
     case SEIST_OP_RES_BWD: return (op.L_out & 3) ? F_RES_BWD : F_RES_BWD4;
     case SEIST_OP_ATT_FWD: return F_ATT_FWD;
@@ -154,7 +137,6 @@ static Family choose(const SeistOp& op) {
     case SEIST_OP_BN_PREPARE_BWD: return F_BN_PREPARE_BWD;
     case SEIST_OP_STEM_COMPOSE_FWD: return F_STEM_COMPOSE_FWD;
     case SEIST_OP_STEM_COMPOSE_BWD: return F_STEM_COMPOSE_BWD;
-    case SEIST_OP_GRAD_COMBINE: return F_GRAD_COMBINE;
     case SEIST_OP_ZERO: return F_ZERO;
     default: return F_NONE;
   }
@@ -190,7 +172,6 @@ static int run_one(const SeistOp& op, cudaStream_t s) {
     case F_BN_PREPARE_BWD: return launch_bn_prepare(op, false, s);
     case F_STEM_COMPOSE_FWD: return launch_stem_compose(op, true, s);
     case F_STEM_COMPOSE_BWD: return launch_stem_compose(op, false, s);
-    case F_GRAD_COMBINE: return launch_grad_combine(op, s, sm_count());
     case F_ZERO: {
       cudaError_t e = cudaMemsetAsync(op.out.x, 0, op.zero_bytes, s);
       if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return (int)e; }

@@ -18,7 +18,6 @@
 // fma2: the gacc rows are parked in shared memory interleaved in channel pairs ({g[2r][s], g[2r+1][s]}), so a
 // 16-byte load yields two aligned (even, odd channel) register pairs; each fma2 multiplies such a pair with one
 // broadcast window sample: 8*K packed FMAs per quad instead of 16*K scalar ones.
-#include <algorithm>
 #include "common.cuh"
 #include "conv_common.cuh"
 
@@ -37,7 +36,7 @@ struct BkOut {
 
 template <int K, int S, int TGM, int NPR>   // NPR pair rows (2*NPR output channels) per thread
 __global__ void __launch_bounds__(BK_NT, (K <= 9 && NPR == 2) ? 3 : 2) bwwk_kernel(const __grid_constant__ SeistOp op, const int CI_B, const int PC,
-                                                        const int pitch, const int area_f, const int gx_off) {
+                                                        const int pitch, const int area_f) {
   constexpr int CO_B = 2 * NPR * TGM;
   constexpr int WN = K + 3 * S, WQ = (WN + 3) / 4;
   constexpr int RW = (K + 1) | 1;                      // odd row pitch of the final fold
@@ -53,8 +52,6 @@ __global__ void __launch_bounds__(BK_NT, (K <= 9 && NPR == 2) ? 3 : 2) bwwk_kern
   float* in_s = g_s + (CO_B / 2) * gpitch;                // [CI_B][pitch]
   BkOut* oc_s = reinterpret_cast<BkOut*>(g_s + area_f);   // [CO_B]
   float* src_s = reinterpret_cast<float*>(oc_s + CO_B);   // [CI_B][width+4] (up-sampled input only)
-  float* gx_s = reinterpret_cast<float*>(sm_raw) + (gx_off > 0 ? gx_off : 0);   // raw x / dxd planes of the asynchronous gacc staging
-  float* gd_s = gx_s + (CO_B / 2) * gpitch;
   const int tid = threadIdx.x;
   const int co_base = grp * gs_out + (blockIdx.y - grp * tpg) * CO_B;
   const int ci_lo = grp * gs_in + blockIdx.z * CI_B;
@@ -109,12 +106,6 @@ __global__ void __launch_bounds__(BK_NT, (K <= 9 && NPR == 2) ? 3 : 2) bwwk_kern
       cp_async_commit();
     }
     // ---- gacc rows, interleaved in channel pairs: g_s[pr][2*s + half] ---------------------------------
-    if (gx_off > 0) {
-      gacc_issue<BK_NT>(op, n, l0, L, co_base, Cout_hi, CO_B, QPR, gpitch, g_s, gx_s, gd_s, has_bn, need_x);
-      cp_async_commit();
-      cp_async_wait<0>();
-      gacc_combine<BK_NT>(op, n, l0, L, co_base, Cout_hi, CO_B, QPR, gpitch, g_s, gx_s, gd_s, oc_s, has_bn, need_x, pf, seed, op.Cout);
-    } else
     for (int idx = tid; idx < (CO_B / 2) * QPR; idx += BK_NT) {
       const int pr = idx / QPR, q = idx - pr * QPR;
       const int l = l0 + 4 * q;
@@ -248,31 +239,16 @@ static int launch_bwwk_t(const SeistOp& op, cudaStream_t s, int sm_count) {
   area_f = (area_f + 3) & ~3;
   size_t smem = sizeof(float) * (size_t)area_f + sizeof(BkOut) * CO_B +
                 (op.up_src_L > 0 ? sizeof(float) * (size_t)CI_B * (width + 4) : 0) + 16;
-  // raw planes of the asynchronous gacc staging (x, dxd next to du) - unless they would cost a resident CTA
-  int gx_off = 0;
-  if (env_knob("SEIST_ASYNC", 7) & 8) {   // opt-in: it helps the row-tiled kernel more than this one
-    const bool has_bn = op.out.bn >= 0 && op.out.g != nullptr;
-    const bool need_x = has_bn || op.out_act == SEIST_OUT_SIGMOID;
-    const int planes = (need_x ? 1 : 0) + ((has_bn && op.out_dxd != nullptr) ? 1 : 0);
-    const size_t base = (smem + 15) & ~(size_t)15;
-    const size_t extra = sizeof(float) * (size_t)planes * (CO_B / 2) * (2 * PC + 8);
-    auto ctas = [](size_t b) { return (227 * 1024) / (b + 1024); };
-    const size_t cap = (K <= 9 && NPR == 2) ? 3 : 2;      // __launch_bounds__ of the kernel
-    if (std::min(cap, ctas(base + extra)) >= std::min(cap, ctas(base))) {
-      gx_off = (int)(base / sizeof(float));
-      smem = base + extra;
-    }
-  }
   const int gy = op.groups * ((gs_out + CO_B - 1) / CO_B), gz = ntile;
   const long tiles = (long)op.N * ((op.L_out + PC - 1) / PC);
-  long gx = ((long)bww_waves() * sm_count + gy * gz - 1) / (gy * gz);
+  long gx = ((long)BWW_WAVES * sm_count + gy * gz - 1) / (gy * gz);
   if (gx > tiles) gx = tiles;
   if (gx < 1) gx = 1;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(bwwk_kernel<K, S, TGM, NPR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
-  bwwk_kernel<K, S, TGM, NPR><<<dim3((unsigned)gx, gy, gz), BK_NT, smem, s>>>(op, CI_B, PC, pitch, area_f, gx_off);
+  bwwk_kernel<K, S, TGM, NPR><<<dim3((unsigned)gx, gy, gz), BK_NT, smem, s>>>(op, CI_B, PC, pitch, area_f);
   note_launch();
   return check_launch("bwwk");
 }

@@ -13,10 +13,11 @@ namespace seist {
 
 // ---- launch bookkeeping (api.cu) -------------------------------------------------------------
 void note_launch();
-int bww_waves();   // resident CTAs per SM the persistent weight-gradient kernels are sized for (SEIST_BWW_WAVES, default 2)
-int env_knob(const char* name, int def);   // integer tuning knob from the environment (measurement only)
 int check_launch(const char* what);
 void set_error(const char* msg);
+
+// resident CTAs per SM the persistent weight-gradient grids (bww, bwwk) are sized for
+constexpr int BWW_WAVES = 2;
 
 // ---- math -------------------------------------------------------------------------------------
 // Two-lane fp32 helpers.  Hopper has no packed fp32 instructions, so each lane is one scalar IEEE operation; the
@@ -289,10 +290,6 @@ __device__ __forceinline__ const float* bn_coef_row(const SeistOp& op, int bn, i
 }
 __device__ __forceinline__ void view_coef(const SeistOp& op, const SeistView& v, int c, float& sc, float& sh) {
   if (v.bn >= 0) {
-    if (op.bn_table[v.bn].inline_coef) {
-      bn_fwd_coef(op.bn_table, v.bn, v.bn_c0 + c, sc, sh);     // once per channel per CTA: cheaper than a launch per BN
-      return;
-    }
     const float2 k = *reinterpret_cast<const float2*>(bn_coef_row(op, v.bn, v.bn_c0 + c));
     sc = k.x;
     sh = k.y;
@@ -309,10 +306,6 @@ struct OutGradCoef {
 __device__ __forceinline__ OutGradCoef out_grad_coef(const SeistOp& op, int co) {
   OutGradCoef k;
   if (op.out.bn >= 0 && op.out.g != nullptr) {
-    if (op.bn_table[op.out.bn].inline_coef) {
-      bn_bwd_coef(op.bn_table, op.out.bn, op.out.bn_c0 + co, k.A, k.Bx, k.Cc);
-      return k;
-    }
     const float4 t = *reinterpret_cast<const float4*>(bn_coef_row(op, op.out.bn, op.out.bn_c0 + co) + 4);
     k.A = t.x;
     k.Bx = t.y;
@@ -339,10 +332,6 @@ __device__ __forceinline__ float out_grad_at(const SeistOp& op, const OutGradCoe
 
 // khat = (x - mu) * istd of the BN applied by view v
 __device__ __forceinline__ void view_khat(const SeistOp& op, const SeistView& v, int c, float& mu, float& istd) {
-  if (op.bn_table[v.bn].inline_coef) {
-    bn_khat_coef(op.bn_table, v.bn, v.bn_c0 + c, mu, istd);
-    return;
-  }
   const float2 k = *reinterpret_cast<const float2*>(bn_coef_row(op, v.bn, v.bn_c0 + c) + 2);
   mu = k.x;
   istd = k.y;

@@ -564,8 +564,6 @@ static int pick_wc(int channels) { return channels > 32 ? 8 : (channels > 16 ? 4
 
 // two stages (asynchronous prefetch of the next reduction chunk) where they do not cost a resident CTA below 2 per SM
 static int ck_pick_nbuf(size_t bytes1, size_t bytes2) {
-  const int knob = env_knob("SEIST_CK_NBUF", 0);
-  if (knob == 1 || knob == 2) return bytes2 > 220 * 1024 ? 1 : knob;
   // the second stage costs a resident CTA on most layers of the model family, which loses more than the prefetch wins:
   // two stages only where they are free
   auto ctas = [](size_t b) { return (int)std::min<size_t>(3, (227 * 1024) / (b + 1024)); };

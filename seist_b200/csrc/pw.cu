@@ -27,13 +27,6 @@ __device__ __forceinline__ float4 lds4(uint32_t a) {
   return v;
 }
 
-// quad group g of this CTA.  G > 0: the CTA owns G consecutive groups (grid = groups / G).  G < 0: "persistent" launch, the
-// grid is exactly the number of CTAs resident at once and a CTA walks the groups blockIdx.x, blockIdx.x + gridDim.x, ...
-// (-G of them): no partially filled last wave, and the CTAs running together touch one contiguous region
-__device__ __forceinline__ long long pw_group(int g, int G) {
-  return G > 0 ? (long long)blockIdx.x * G + g : (long long)blockIdx.x + (long long)g * gridDim.x;
-}
-
 struct PwChan {          // one reduction / target channel, resolved once per CTA
   const float* x;        // row base for n = 0
   float* g;              // gradient row base for n = 0 (backward targets) or nullptr
@@ -214,10 +207,7 @@ __device__ __noinline__ float4 pw_keep4(float p, uint64_t seed, uint32_t stream,
 
 // compile-time specialisation keeps the bodies small (instruction cache) and the inner loops free of
 // runtime feature tests: F_ELEM element dropout, F_RES residual views, F_GELU some view applies GELU
-constexpr int PWF_CG = 4;                                    // reduction channels per ring stage
-constexpr int PWF_S = 3;                                     // stages (PWF_S - 1 steps in flight)
-constexpr int PWF_STAGE_B = PWF_CG * PW_NT * 16;             // [channel][thread] float4
-template <int COUT_T, bool F_ELEM, bool F_RES, bool F_GELU, bool F_POOL = false, bool RING = false>
+template <int COUT_T, bool F_ELEM, bool F_RES, bool F_GELU, bool F_POOL = false>
 __global__ void __launch_bounds__(PW_NT, 4) pw_fwd_kernel(const __grid_constant__ SeistOp op, const int G) {
   extern __shared__ __align__(16) unsigned char sm_raw[];
   const int Cin = op.Cin, Cin8 = (Cin + 7) & ~7;
@@ -227,7 +217,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_fwd_kernel(const __grid_constant_
   float* red_s = ep_s + 5 * COUT_T;                                       // [4][2*COUT_T]
   float* st_s = red_s + 4 * 2 * COUT_T;                                   // [4 warps][2*COUT_T][32 lanes] running sums
   const int tid = threadIdx.x;
-  const uint32_t ring = smem_addr(st_s + 4 * 2 * COUT_T * 32) + tid * 16;  // RING: [PWF_S] stages (16-byte aligned carve-up)
   const int co_base = blockIdx.y * COUT_T;
   const int L = op.L_out, LQ = L >> 2;
 
@@ -263,7 +252,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_fwd_kernel(const __grid_constant_
 
   const uint64_t seed = load_seed(op.step_seed);
   const long long NQ = (long long)op.N * LQ;
-  const int Gn = G < 0 ? -G : G;
   const bool stats = (op.out.bn >= 0) && op.bn_table[op.out.bn >= 0 ? op.out.bn : 0].use_batch;
   // BatchNorm sums of the result live in shared memory (one private slot per thread and statistic) between
   // quads: in registers they would cost 2*COUT_T registers across the whole contraction loop
@@ -271,40 +259,8 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_fwd_kernel(const __grid_constant_
 #pragma unroll
   for (int i = 0; i < 2 * COUT_T; ++i) my_st[i * 32] = 0.f;
 
-  // RING: the operands of the contraction travel through a per-thread asynchronous copy ring, PWF_S - 1 steps of
-  // PWF_CG channels ahead of their use and across quad groups (see pw_bwd_data_kernel)
-  int ig = 0, ici = 0, istage = 0, cstage = 0, in_n = 0, in_l = 0;
-  auto quad_nl = [&](int g, int& n, int& l) {
-    const long long f = pw_group(g, G) * PW_NT + tid;
-    const bool ok = f < NQ;
-    n = ok ? (int)(f / LQ) : 0;
-    l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
-  };
-  auto issue_step = [&]() {
-    if (ig < Gn) {
-      const uint32_t dst0 = ring + istage * PWF_STAGE_B;
-#pragma unroll
-      for (int j = 0; j < PWF_CG; ++j) {
-        const PwChan& c = ch_s[ici + j];
-        cp_async16(dst0 + j * (PW_NT * 16), c.x + (long long)in_n * c.nstride + in_l);
-      }
-      ici += PWF_CG;
-      if (ici >= Cin8) {
-        ici = 0;
-        if (++ig < Gn) quad_nl(ig, in_n, in_l);
-      }
-    }
-    cp_async_commit();
-    istage = istage + 1 == PWF_S ? 0 : istage + 1;
-  };
-  if constexpr (RING) {
-    quad_nl(0, in_n, in_l);
-#pragma unroll
-    for (int s = 0; s < PWF_S - 1; ++s) issue_step();
-  }
-
-  for (int g = 0; g < Gn; ++g) {
-    const long long f = pw_group(g, G) * PW_NT + tid;
+  for (int g = 0; g < G; ++g) {
+    const long long f = ((long long)blockIdx.x * G + g) * PW_NT + tid;
     const bool ok = f < NQ;
     const int n = ok ? (int)(f / LQ) : 0;
     const int l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
@@ -313,30 +269,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_fwd_kernel(const __grid_constant_
     for (int c = 0; c < COUT_T / 2; ++c)
 #pragma unroll
       for (int q = 0; q < 4; ++q) acc[c][q] = make_float2(0.f, 0.f);
-    if constexpr (RING) {
-      for (int ci0 = 0; ci0 < Cin8; ci0 += PWF_CG) {
-        issue_step();
-        cp_async_wait<PWF_S - 1>();
-        const uint32_t src0 = ring + cstage * PWF_STAGE_B;
-        cstage = cstage + 1 == PWF_S ? 0 : cstage + 1;
-#pragma unroll
-        for (int j = 0; j < PWF_CG; ++j) {
-          const PwChan& c = ch_s[ci0 + j];
-          float4 u = apply_view(lds4(src0 + j * (PW_NT * 16)), c.sc, c.sh, 0);
-          if (F_GELU && c.act == SEIST_ACT_GELU) u = pw_gelu4(u);
-          const float2* wr = reinterpret_cast<const float2*>(w_s + (ci0 + j) * COUT_T);
-          const float2 ux = dup2(u.x), uy = dup2(u.y), uz = dup2(u.z), uw = dup2(u.w);
-#pragma unroll
-          for (int cp = 0; cp < COUT_T / 2; ++cp) {
-            const float2 w = wr[cp];
-            acc[cp][0] = fma2(w, ux, acc[cp][0]);
-            acc[cp][1] = fma2(w, uy, acc[cp][1]);
-            acc[cp][2] = fma2(w, uz, acc[cp][2]);
-            acc[cp][3] = fma2(w, uw, acc[cp][3]);
-          }
-        }
-      }
-    } else
     for (int ci0 = 0; ci0 < Cin8; ci0 += 8) {
       float4 v[8];
 #pragma unroll
@@ -458,8 +390,9 @@ struct PwOut {   // per output channel of the forward op, resolved once per CTA
 
 constexpr int PW_RING_S = 3;                                   // ring stages (PW_RING_S - 1 contraction steps in flight)
 constexpr int PW_RING_STAGE_B = PW_BD_CG * 3 * PW_NT * 16;     // bytes per stage: [channel][dxd | du | x][thread] float4
-template <int CI_T, bool F_ELEM, bool F_GELU, bool F_POOL = false, bool RING = false>
-__global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_constant__ SeistOp op, const int G, const int pre) {
+template <int CI_T, bool F_ELEM, bool F_GELU, bool F_POOL = false>
+__global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_constant__ SeistOp op, const int G) {
+  constexpr bool RING = !F_POOL;   // the pooled instantiation loads its operands directly
   extern __shared__ __align__(16) unsigned char sm_raw[];
   const int Cout = op.Cout, Cout4 = (Cout + 3) & ~3, Cin = op.Cin;
   PwChan* ch_s = reinterpret_cast<PwChan*>(sm_raw);                       // [CI_T] targets
@@ -470,11 +403,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
   const int tid = threadIdx.x;
   // RING: [PW_RING_S] stages behind the statistics (16-byte aligned: every carve-up above is a multiple of 16 bytes)
   const uint32_t ring = smem_addr(st_s + 4 * 2 * CI_T * 32) + tid * 16;
-  // epilogue operands of the targets (x for khat / GELU' [pre & 1], the old gradient when accumulating [pre & 2]):
-  // copied asynchronously at the start of a quad group, so that their latency hides behind the contraction loop
-  // instead of being exposed once per batch of PW_BD_EB channels.  [plane][CI_T][thread] float4
-  const uint32_t pre_x = ring + (RING ? PW_RING_S * PW_RING_STAGE_B : 0);
-  const uint32_t pre_o = pre_x + ((pre & 1) ? CI_T * PW_NT * 16 : 0);
   const int ci_base = blockIdx.y * CI_T;
   const int L = op.L_out, LQ = L >> 2;
 
@@ -503,7 +431,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
 
   const uint64_t seed = load_seed(op.step_seed);
   const long long NQ = (long long)op.N * LQ;
-  const int Gn = G < 0 ? -G : G;
   const bool has_bn = (op.out.bn >= 0 && op.out.g != nullptr);
   const bool need_x = has_bn || op.out_act == SEIST_OUT_SIGMOID;
   // BN-backward sums of the targets live in shared memory (one private slot per thread and statistic)
@@ -517,14 +444,14 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
   int ig = 0, ico = 0, istage = 0, cstage = 0;
   size_t iobase = 0;
   auto quad_base = [&](int g) -> size_t {
-    const long long f = pw_group(g, G) * PW_NT + tid;
+    const long long f = ((long long)blockIdx.x * G + g) * PW_NT + tid;
     const bool ok = f < NQ;
     const int n = ok ? (int)(f / LQ) : 0;
     const int l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
     return ((size_t)n * op.out.Ct + op.out.c0) * (size_t)L + l;
   };
   auto issue_step = [&]() {
-    if (ig < Gn) {
+    if (ig < G) {
       const uint32_t dst0 = ring + istage * PW_RING_STAGE_B;
 #pragma unroll
       for (int j = 0; j < PW_BD_CG; ++j) {
@@ -537,7 +464,7 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
       ico += PW_BD_CG;
       if (ico >= Cout4) {
         ico = 0;
-        if (++ig < Gn) iobase = quad_base(ig);
+        if (++ig < G) iobase = quad_base(ig);
       }
     }
     cp_async_commit();   // one group per step (possibly empty) keeps the wait count uniform
@@ -549,8 +476,8 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
     for (int s = 0; s < PW_RING_S - 1; ++s) issue_step();
   }
 
-  for (int g = 0; g < Gn; ++g) {
-    const long long f = pw_group(g, G) * PW_NT + tid;
+  for (int g = 0; g < G; ++g) {
+    const long long f = ((long long)blockIdx.x * G + g) * PW_NT + tid;
     const bool ok = f < NQ;
     const int n = ok ? (int)(f / LQ) : 0;
     const int l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
@@ -561,17 +488,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
 #pragma unroll
       for (int q = 0; q < 4; ++q) acc[c][q] = make_float2(0.f, 0.f);
     const size_t obase = ((size_t)n * op.out.Ct + op.out.c0) * (size_t)L + l;
-    if (!F_POOL && pre && ok) {
-#pragma unroll
-      for (int col = 0; col < CI_T; ++col) {
-        const PwChan& c = ch_s[col];
-        if (c.g == nullptr) continue;
-        const long long off = (long long)n * c.nstride + l;
-        if ((pre & 1) && ((F_GELU && c.act == SEIST_ACT_GELU) || c.bn >= 0)) cp_async16(pre_x + col * (PW_NT * 16), c.x + off);
-        if ((pre & 2) && c.accum) cp_async16(pre_o + col * (PW_NT * 16), c.g + off);
-      }
-      cp_async_commit();
-    }
     for (int co0 = 0; co0 < Cout4; co0 += PW_BD_CG) {
       float4 dx[PW_BD_CG], du[PW_BD_CG], xo[PW_BD_CG];
       if constexpr (RING) {
@@ -659,7 +575,6 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
     // targets in batches of PW_BD_EB channels: all loads of a batch (x for khat / GELU', the old gradient when
     // accumulating) are issued before its first store, so their latency overlaps instead of serialising
     // load -> use -> store once per channel (the compiler cannot hoist loads over possibly aliasing stores)
-    if (pre) cp_async_wait<0>();
 #pragma unroll
     for (int cb = 0; cb < CI_T; cb += PW_BD_EB) {
       float4 xv[PW_BD_EB], ov[PW_BD_EB];
@@ -669,10 +584,8 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
         const long long off = (long long)n * c.nstride + l;
         const bool live = c.g != nullptr;
         const bool want_x = live && ((F_GELU && c.act == SEIST_ACT_GELU) || c.bn >= 0);
-        if (pre & 1) xv[u] = want_x ? lds4(pre_x + (cb + u) * (PW_NT * 16)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        else xv[u] = want_x ? ldg4(c.x + off) : make_float4(0.f, 0.f, 0.f, 0.f);
-        if (pre & 2) ov[u] = (live && c.accum) ? lds4(pre_o + (cb + u) * (PW_NT * 16)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        else ov[u] = (live && c.accum) ? ld4(c.g + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+        xv[u] = want_x ? ldg4(c.x + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+        ov[u] = (live && c.accum) ? ld4(c.g + off) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
 #pragma unroll
       for (int u = 0; u < PW_BD_EB; ++u) {
@@ -725,7 +638,6 @@ __global__ void __launch_bounds__(PW_NT) res_bwd4_kernel(const __grid_constant__
   const int co = blockIdx.y;
   const int L = op.L_out, LQ = L >> 2;
   const long long NQ = (long long)op.N * LQ;
-  const int Gn = G < 0 ? -G : G;
   const uint64_t seed = load_seed(op.step_seed);
   const OutGradCoef kc = out_grad_coef(op, co);
   const bool has_bn = (op.out.bn >= 0 && op.out.g != nullptr);
@@ -737,8 +649,8 @@ __global__ void __launch_bounds__(PW_NT) res_bwd4_kernel(const __grid_constant__
   if (wa && va.bn >= 0) view_khat(op, va, co, amu, aistd);
   if (wb && vb.bn >= 0) view_khat(op, vb, co, bmu, bistd);
   float st[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int g = 0; g < Gn; ++g) {
-    const long long f = pw_group(g, G) * PW_NT + tid;
+  for (int g = 0; g < G; ++g) {
+    const long long f = ((long long)blockIdx.x * G + g) * PW_NT + tid;
     if (f >= NQ) break;
     const int n = (int)(f / LQ);
     const int l = (int)(f - (long long)n * LQ) * 4;
@@ -819,11 +731,10 @@ bool pw_eligible(const SeistOp& op) {
 }
 
 static int pick_G(long long nq, int tiles_y, int sm_count) {
-  // enough CTAs for ~4 waves, but several quads per thread to amortise the per-CTA setup / reduction
+  // enough CTAs for ~4 waves, but several quads per thread (at most 8) to amortise the per-CTA setup / reduction
   long long ctas = (nq + PW_NT - 1) / PW_NT;
   int G = 1;
-  const int gmax = env_knob("SEIST_PW_GMAX", 8);
-  while (G < gmax && (ctas / (2 * G)) * tiles_y >= 4LL * sm_count) G *= 2;
+  while (G < 8 && (ctas / (2 * G)) * tiles_y >= 4LL * sm_count) G *= 2;
   return G;
 }
 
@@ -836,55 +747,21 @@ static int pw_set_smem(K kernel, size_t bytes) {
   return 0;
 }
 
-// persistent sizing of the streaming kernels (see pw_group): exactly the CTAs resident at once, each walking
-// ceil(groups / grid) quad groups.  The former "G consecutive groups per CTA" grids ended in a partially filled
-// wave (typically 1.7 - 2.6 waves).  SEIST_PW_PERSIST=1 enables it (A/B runs; it did not pay, see below).
-static thread_local int tl_sm_count = 0;
-static thread_local long long tl_groups = 0;
-template <typename K>
-static void pw_persist(K kernel, size_t smem, dim3& grid, int& G) {
-  if (!env_knob("SEIST_PW_PERSIST", 0) || tl_sm_count <= 0) return;   // opt-in
-  int nb = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, PW_NT, smem) != cudaSuccess || nb < 1) return;
-  long long gx = (long long)nb * tl_sm_count / grid.y;
-  if (gx < 1) gx = 1;
-  if (gx >= tl_groups) {
-    grid.x = (unsigned)tl_groups;
-    G = 1;
-    return;
-  }
-  grid.x = (unsigned)gx;
-  G = -(int)((tl_groups + gx - 1) / gx);
-}
-
 static bool any_gelu(const SeistOp& op) {
   for (int i = 0; i < op.n_in; ++i)
     if (op.in[i].act == SEIST_ACT_GELU) return true;
   return false;
 }
 
-template <int COT, bool E, bool R, bool Gf>
+template <int COT, bool E, bool R, bool Gf, bool P = false>
 static int pw_fwd_go(const SeistOp& op, cudaStream_t s, dim3 grid, size_t smem, int G) {
-  if (env_knob("SEIST_PW_RING", 1) & 2) {
-    smem += (size_t)PWF_S * PWF_STAGE_B;
-    int rc = pw_set_smem(pw_fwd_kernel<COT, E, R, Gf, false, true>, smem);
-    pw_persist(pw_fwd_kernel<COT, E, R, Gf, false, true>, smem, grid, G);
-    if (!rc) pw_fwd_kernel<COT, E, R, Gf, false, true><<<grid, PW_NT, smem, s>>>(op, G);
-    return rc;
-  }
-  int rc = pw_set_smem(pw_fwd_kernel<COT, E, R, Gf>, smem);
-    pw_persist(pw_fwd_kernel<COT, E, R, Gf>, smem, grid, G);
-  if (!rc) pw_fwd_kernel<COT, E, R, Gf><<<grid, PW_NT, smem, s>>>(op, G);
+  int rc = pw_set_smem(pw_fwd_kernel<COT, E, R, Gf, P>, smem);
+  if (!rc) pw_fwd_kernel<COT, E, R, Gf, P><<<grid, PW_NT, smem, s>>>(op, G);
   return rc;
 }
 template <int COT>
 static int pw_fwd_sel(const SeistOp& op, cudaStream_t s, dim3 grid, size_t smem, int G) {
-  if (op.pool > 1) {
-    int rc = pw_set_smem(pw_fwd_kernel<COT, false, false, false, true>, smem);
-    pw_persist(pw_fwd_kernel<COT, false, false, false, true>, smem, grid, G);
-    if (!rc) pw_fwd_kernel<COT, false, false, false, true><<<grid, PW_NT, smem, s>>>(op, G);
-    return rc;
-  }
+  if (op.pool > 1) return pw_fwd_go<COT, false, false, false, true>(op, s, grid, smem, G);
   const int sel = (op.p_elem > 0.f ? 4 : 0) | ((op.res_a.C > 0 || op.res_b.C > 0) ? 2 : 0) | (any_gelu(op) ? 1 : 0);
   switch (sel) {
     case 0: return pw_fwd_go<COT, false, false, false>(op, s, grid, smem, G);
@@ -906,51 +783,28 @@ int launch_pw_fwd(const SeistOp& op, cudaStream_t s, int sm_count) {
   const int ty = (op.Cout + cot - 1) / cot;
   const int G = pick_G(nq, ty, sm_count);
   dim3 grid((unsigned)((nq + (long long)PW_NT * G - 1) / ((long long)PW_NT * G)), ty);
-  tl_sm_count = sm_count;
-  tl_groups = (nq + PW_NT - 1) / PW_NT;
   const int rc = cot == 16 ? pw_fwd_sel<16>(op, s, grid, smem, G) : pw_fwd_sel<8>(op, s, grid, smem, G);
   if (rc) return rc;
   note_launch();
   return check_launch("pw_fwd");
 }
 
-template <int CIT, bool E, bool Gf>
-static int pw_bwdd_go(const SeistOp& op, cudaStream_t s, dim3 grid, size_t smem, int G, int pre) {
-  if (env_knob("SEIST_PW_RING", 1) & 1) {
-    smem += (size_t)PW_RING_S * PW_RING_STAGE_B;
-    int rc = pw_set_smem(pw_bwd_data_kernel<CIT, E, Gf, false, true>, smem);
-    pw_persist(pw_bwd_data_kernel<CIT, E, Gf, false, true>, smem, grid, G);
-    if (!rc) pw_bwd_data_kernel<CIT, E, Gf, false, true><<<grid, PW_NT, smem, s>>>(op, G, 0);
-    return rc;
-  }
-  smem += (size_t)((pre & 1) + ((pre >> 1) & 1)) * CIT * PW_NT * 16;
-  int rc = pw_set_smem(pw_bwd_data_kernel<CIT, E, Gf>, smem);
-    pw_persist(pw_bwd_data_kernel<CIT, E, Gf>, smem, grid, G);
-  if (!rc) pw_bwd_data_kernel<CIT, E, Gf><<<grid, PW_NT, smem, s>>>(op, G, pre);
+template <int CIT, bool E, bool Gf, bool P = false>
+static int pw_bwdd_go(const SeistOp& op, cudaStream_t s, dim3 grid, size_t smem, int G) {
+  if (!P) smem += (size_t)PW_RING_S * PW_RING_STAGE_B;   // operand ring
+  int rc = pw_set_smem(pw_bwd_data_kernel<CIT, E, Gf, P>, smem);
+  if (!rc) pw_bwd_data_kernel<CIT, E, Gf, P><<<grid, PW_NT, smem, s>>>(op, G);
   return rc;
 }
 template <int CIT>
 static int pw_bwdd_sel(const SeistOp& op, cudaStream_t s, dim3 grid, size_t smem, int G) {
-  if (op.pool > 1) {
-    int rc = pw_set_smem(pw_bwd_data_kernel<CIT, false, false, true>, smem);
-    pw_persist(pw_bwd_data_kernel<CIT, false, false, true>, smem, grid, G);
-    if (!rc) pw_bwd_data_kernel<CIT, false, false, true><<<grid, PW_NT, smem, s>>>(op, G, 0);
-    return rc;
-  }
-  // epilogue prefetch planes: bit 0 = some target needs x (BatchNorm khat / GELU'), bit 1 = some target accumulates
-  int pre = 0;
-  for (int i = 0; i < op.n_in; ++i) {
-    if (op.in[i].g == nullptr) continue;
-    if (op.in[i].bn >= 0 || op.in[i].act == SEIST_ACT_GELU) pre |= 1;
-    if (op.in[i].accum) pre |= 2;
-  }
-  pre &= env_knob("SEIST_PW_PRE", 0);   // the prefetch planes cost a resident CTA: opt-in
+  if (op.pool > 1) return pw_bwdd_go<CIT, false, false, true>(op, s, grid, smem, G);
   const int sel = (op.p_elem > 0.f ? 2 : 0) | (any_gelu(op) ? 1 : 0);
   switch (sel) {
-    case 0: return pw_bwdd_go<CIT, false, false>(op, s, grid, smem, G, pre);
-    case 1: return pw_bwdd_go<CIT, false, true>(op, s, grid, smem, G, pre);
-    case 2: return pw_bwdd_go<CIT, true, false>(op, s, grid, smem, G, pre);
-    default: return pw_bwdd_go<CIT, true, true>(op, s, grid, smem, G, pre);
+    case 0: return pw_bwdd_go<CIT, false, false>(op, s, grid, smem, G);
+    case 1: return pw_bwdd_go<CIT, false, true>(op, s, grid, smem, G);
+    case 2: return pw_bwdd_go<CIT, true, false>(op, s, grid, smem, G);
+    default: return pw_bwdd_go<CIT, true, true>(op, s, grid, smem, G);
   }
 }
 
@@ -962,65 +816,10 @@ int launch_pw_bwd_data(const SeistOp& op, cudaStream_t s, int sm_count) {
   const int ty = (op.Cin + cit - 1) / cit;
   const int G = pick_G(nq, ty, sm_count);
   dim3 grid((unsigned)((nq + (long long)PW_NT * G - 1) / ((long long)PW_NT * G)), ty);
-  tl_sm_count = sm_count;
-  tl_groups = (nq + PW_NT - 1) / PW_NT;
   const int rc = cit == 16 ? pw_bwdd_sel<16>(op, s, grid, smem, G) : pw_bwdd_sel<8>(op, s, grid, smem, G);
   if (rc) return rc;
   note_launch();
   return check_launch("pw_bwd_data");
-}
-
-// ================================================================================================
-// GRAD_COMBINE: BatchNorm backward of the output gradient, once and in place (out.g <- A*out.g + Bx*x + Cc
-// [+ dxd]); grid (ceil(NQ/(128*G)), C).  The backward ops of the same conv then read a plain gradient.
-// ================================================================================================
-__global__ void __launch_bounds__(PW_NT) grad_combine_kernel(const __grid_constant__ SeistOp op, const int G) {
-  const int co = blockIdx.y;
-  const int L = op.out.L;
-  const OutGradCoef kc = out_grad_coef(op, co);
-  const size_t row = (size_t)op.out.Ct * L, base = (size_t)(op.out.c0 + co) * L;
-  if ((L & 3) == 0) {
-    const int LQ = L >> 2;
-    const long long NQ = (long long)op.N * LQ;
-    for (int g = 0; g < G; ++g) {
-      const long long f = ((long long)blockIdx.x * G + g) * PW_NT + threadIdx.x;
-      if (f >= NQ) break;
-      const int n = (int)(f / LQ);
-      const int l = (int)(f - (long long)n * LQ) * 4;
-      const size_t off = (size_t)n * row + base + l;
-      const float4 du = ld4(op.out.g + off), x = ldg4(op.out.x + off);
-      float4 r = op.out_dxd ? ldg4(op.out_dxd + off) : make_float4(0.f, 0.f, 0.f, 0.f);
-      r.x += fmaf(kc.A, du.x, fmaf(kc.Bx, x.x, kc.Cc));
-      r.y += fmaf(kc.A, du.y, fmaf(kc.Bx, x.y, kc.Cc));
-      r.z += fmaf(kc.A, du.z, fmaf(kc.Bx, x.z, kc.Cc));
-      r.w += fmaf(kc.A, du.w, fmaf(kc.Bx, x.w, kc.Cc));
-      st4(op.out.g + off, r);
-    }
-  } else {
-    const long long NE = (long long)op.N * L;
-    for (int g = 0; g < 4 * G; ++g) {
-      const long long f = ((long long)blockIdx.x * 4 * G + g) * PW_NT + threadIdx.x;
-      if (f >= NE) break;
-      const int n = (int)(f / L);
-      const size_t off = (size_t)n * row + base + (size_t)(f - (long long)n * L);
-      float r = op.out_dxd ? op.out_dxd[off] : 0.f;
-      r += fmaf(kc.A, op.out.g[off], fmaf(kc.Bx, op.out.x[off], kc.Cc));
-      op.out.g[off] = r;
-    }
-  }
-}
-
-int launch_grad_combine(const SeistOp& op, cudaStream_t s, int sm_count) {
-  if (op.out.bn < 0 || op.out.g == nullptr) {
-    set_error("GRAD_COMBINE: the output view has no BatchNorm gradient");
-    return -4;
-  }
-  const long long nq = ((long long)op.N * op.out.L + 3) / 4;
-  const int G = pick_G(nq, op.out.C, sm_count);
-  dim3 grid((unsigned)((nq + (long long)PW_NT * G - 1) / ((long long)PW_NT * G)), op.out.C);
-  grad_combine_kernel<<<grid, PW_NT, 0, s>>>(op, G);
-  note_launch();
-  return check_launch("grad_combine");
 }
 
 int launch_res_bwd4(const SeistOp& op, cudaStream_t s, int sm_count) {
@@ -1047,7 +846,7 @@ constexpr int BW_NT = 256;
 
 // BW_PC = output samples per chunk (128, or 512 for narrow tiles where the per-chunk barriers/latency dominate)
 template <int CO_B, int R_B, bool K1, int BW_PC>
-__global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ SeistOp op, const int nci_max, const int async_in, const int gx_off) {
+__global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ SeistOp op, const int nci_max, const int g_async, const int gx_off) {
   constexpr int BW_PITCH = BW_PC + 4;   // input row pitch (floats), keeps 16-byte alignment
   constexpr int BW_GP = 2 * BW_PC + 8;  // gacc channel-PAIR row pitch: g_s[pr][2*s + half] (fma2 operand pairs)
   extern __shared__ __align__(16) unsigned char sm_raw[];
@@ -1069,7 +868,7 @@ __global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ S
   PwOut* oc_s = reinterpret_cast<PwOut*>(g_s + ((area_f + 3) & ~3));   // [CO_B]
   PwChan* ch_s = reinterpret_cast<PwChan*>(oc_s + CO_B);                // [nci_max] (k = 1 fast path)
   float* src_s = reinterpret_cast<float*>(ch_s + nci_max + 1);          // [nci_max][width+4] (up-sampled input only)
-  float* gx_s = reinterpret_cast<float*>(sm_raw) + gx_off;              // [2][CO_B/2][BW_GP] raw x / dxd planes (async_in & 2)
+  float* gx_s = reinterpret_cast<float*>(sm_raw) + gx_off;              // [2][CO_B/2][BW_GP] raw x / dxd planes (g_async)
   float* gd_s = gx_s + (CO_B / 2) * BW_GP;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int co_base = grp * gs_out + (blockIdx.y - grp * tpg) * CO_B, r_base = blockIdx.z * R_B;
@@ -1126,7 +925,7 @@ __global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ S
     // ---- conv-input rows, k = 1 fast path: raw 16-byte asynchronous copies, ALL in flight at once and behind the
     // gacc loads below; every thread later transforms its own quads in place (no barrier in between).  A
     // load -> transform -> store loop would expose one memory latency per quad
-    const bool in_async = K1 && vec && plain && async_in;
+    const bool in_async = K1 && vec && plain;
     if (in_async) {
       for (int idx = tid; idx < nci * QPR; idx += BW_NT) {
         const int row = idx / QPR, q = idx - row * QPR;
@@ -1142,8 +941,7 @@ __global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ S
       cp_async_commit();
     }
     // ---- gacc rows ------------------------------------------------------------------------------
-    const bool g_async = vec && (async_in & 2);
-    if (g_async) {
+    if (vec && g_async) {
       gacc_issue<BW_NT>(op, n, l0, L, co_base, Cout, CO_B, QPR, BW_GP, g_s, gx_s, gd_s, has_bn, need_x);
       cp_async_commit();
       cp_async_wait<0>();
@@ -1216,17 +1014,6 @@ __global__ void __launch_bounds__(BW_NT, 3) bww_kernel(const __grid_constant__ S
           float* dst = in_s + row * pitch + 4 * q;
           st4(dst, apply_view2(ld4(dst), c.sc, c.sh, c.act));
         }
-      }
-    } else if (K1 && vec && plain) {
-      for (int idx = tid; idx < nci * QPR; idx += BW_NT) {
-        const int row = idx / QPR, q = idx - row * QPR;
-        const int l = l0 + 4 * q;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (l < L) {
-          const PwChan& c = ch_s[row];
-          v = apply_view(ldg4(c.x + (long long)n * c.nstride + l), c.sc, c.sh, c.act);
-        }
-        st4(in_s + row * pitch + 4 * q, v);
       }
     } else {
       if (op.up_src_L > 0) {
@@ -1329,27 +1116,23 @@ static int launch_bww_pc(const SeistOp& op, cudaStream_t s, int sm_count) {
   size_t smem = sizeof(float) * (size_t)((stage_f + 3) & ~3) + sizeof(PwOut) * CO_B + sizeof(PwChan) * (nci_max + 1) + 64 +
                 (op.up_src_L > 0 ? sizeof(float) * (size_t)nci_max * (width + 4) : 0);
   // raw planes of the asynchronous gacc staging (x, dxd next to du) - unless they would cost the second resident CTA
-  int async = env_knob("SEIST_ASYNC", 7);
   smem = (smem + 15) & ~(size_t)15;
   const int gx_off = (int)(smem / sizeof(float));
-  {
-    const bool has_bn = op.out.bn >= 0 && op.out.g != nullptr;
-    const bool need_x = has_bn || op.out_act == SEIST_OUT_SIGMOID;
-    const int planes = (need_x ? 1 : 0) + ((has_bn && op.out_dxd != nullptr) ? 1 : 0);
-    const size_t extra = sizeof(float) * (size_t)planes * (CO_B / 2) * (2 * BW_PC + 8);
-    const bool vec = (op.L_out & 3) == 0;
-    if (!vec || (smem <= 113 * 1024 && smem + extra > 113 * 1024)) async &= ~2;
-    if (async & 2) smem += extra;
-  }
+  const bool has_bn = op.out.bn >= 0 && op.out.g != nullptr;
+  const bool need_x = has_bn || op.out_act == SEIST_OUT_SIGMOID;
+  const int planes = (need_x ? 1 : 0) + ((has_bn && op.out_dxd != nullptr) ? 1 : 0);
+  const size_t extra = sizeof(float) * (size_t)planes * (CO_B / 2) * (2 * BW_PC + 8);
+  const bool g_async = (op.L_out & 3) == 0 && !(smem <= 113 * 1024 && smem + extra > 113 * 1024);
+  if (g_async) smem += extra;
   const int R = (op.Cin / op.groups) * k;
   const int gy = op.groups * ((op.Cout / op.groups + CO_B - 1) / CO_B), gz = (R + R_B - 1) / R_B;
   const long tiles = (long)op.N * ((op.L_out + BW_PC - 1) / BW_PC);
-  long gx = ((long)bww_waves() * sm_count + gy * gz - 1) / (gy * gz);
+  long gx = ((long)BWW_WAVES * sm_count + gy * gz - 1) / (gy * gz);
   if (gx > tiles) gx = tiles;
   if (gx < 1) gx = 1;
   int rc = pw_set_smem(bww_kernel<CO_B, R_B, K1, BW_PC>, smem);
   if (rc) return rc;
-  bww_kernel<CO_B, R_B, K1, BW_PC><<<dim3((unsigned)gx, gy, gz), BW_NT, smem, s>>>(op, nci_max, async & 3, gx_off);
+  bww_kernel<CO_B, R_B, K1, BW_PC><<<dim3((unsigned)gx, gy, gz), BW_NT, smem, s>>>(op, nci_max, g_async ? 1 : 0, gx_off);
   note_launch();
   return check_launch("bww");
 }

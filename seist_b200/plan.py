@@ -14,7 +14,6 @@ Reference semantics cited per emitter (paths relative to the reference's models/
 from __future__ import annotations
 
 import ctypes
-import os
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
@@ -121,7 +120,6 @@ class Op:
     n_bn: int = 0
     name: str = ""
     fwd: Optional["Op"] = None            # backward ops point at their forward op
-    combined: bool = False                # forward op whose output gradient is BN-backward-combined in place (GRAD_COMBINE)
     sync_bn: List[int] = field(default_factory=list)  # BN indices whose (g)stat must be all-reduced BEFORE this op
 
 
@@ -223,10 +221,6 @@ class PlanBuilder:
         self.plan = Plan()
         self.mods = dict(model.named_modules())
         self.seed_ctr = 1
-        # SEIST_BN_INLINE=1 (single-GPU training): no BN_PREPARE launches (216 per seist_m_dpk step), every consumer CTA
-        # derives the per-channel coefficients from the statistics while it resolves its views.  The fp64 divisions / rsqrt
-        # repeated by every CTA cost more than the launches they save, so the separate launches stay the default.
-        self.inline_coef = bool(training and world == 1 and os.environ.get("SEIST_BN_INLINE", "0") == "1")
         self._bn_idx: Dict[str, int] = {}
         self._st_off = 0
         self._wx_off = 0
@@ -471,7 +465,6 @@ class PlanBuilder:
     def build(self) -> Plan:
         hp, pl = self.hp, self.plan
         pl.N, pl.L, pl.training, pl.world, pl.device, pl.flat = self.N, self.Lx, self.training, self.world, self.device, self.flat
-        pl.inline_coef = self.inline_coef
         xin = self.buf("x", hp.in_channels, self.Lx, no_grad=True)
         pl.x_in = xin
         cur = View(xin, 0, hp.in_channels)
@@ -526,9 +519,6 @@ class PlanBuilder:
         for f in reversed(pl.fwd_ops):
             if f.kind == _lib.CONV_FWD:
                 up_atomic = f.up_src_L > 0
-                if self._wants_combine(f):
-                    f.combined = True
-                    ops.append(Op(_lib.GRAD_COMBINE, f.N, out=f.out, fwd=f, name=f.name + ":gcomb"))
                 if f.res_a is not None or f.res_b is not None:
                     ra, rb = grad_target(f.res_a), grad_target(f.res_b)
                     if ra is not None or rb is not None:
@@ -557,17 +547,6 @@ class PlanBuilder:
                 pass
         ops.append(Op(_lib.BN_FINALIZE_BWD, self.N, name="bn_finalize_bwd"))
 
-    @staticmethod
-    def _wants_combine(f: Op) -> bool:
-        """Evaluate the BN backward of f's output once (GRAD_COMBINE) instead of in every pass of its three
-        backward ops?  Pays off when the data gradient needs several 16-channel passes over the output gradient
-        (wide 1x1 convs): each pass then loads one tensor instead of (du, x[, dxd]).  The combine passes cost about
-        what the backward ops save, so it is OFF by default; SEIST_COMBINE_CIN=<min reduction width> enables it."""
-        thr = int(os.environ.get("SEIST_COMBINE_CIN", "0"))
-        if thr <= 0 or f.out is None or f.out.bn < 0 or not f.out.buf.need_du:
-            return False
-        return f.k == 1 and f.stride == 1 and f.groups == 1 and f.Cin >= thr
-
     def _insert_prepares(self, ops: List[Op], forward: bool) -> List[Op]:
         """Insert the BN_PREPARE ops: the per-channel coefficient table of a BN is computed once, after its
         last producer and before its first consumer (forward: scale/shift/khat from the batch statistics;
@@ -577,8 +556,6 @@ class PlanBuilder:
         nb = len(self.plan.bns)
         if forward and not self.training:
             return [Op(kind, self.N, bn_lo=0, n_bn=nb, name="bn_prepare_all")] + ops
-        if self.inline_coef:
-            return ops          # single-GPU training: the consumers derive the coefficients themselves (SeistBN.inline_coef)
         out: List[Op] = []
         ready = set()
         for op in ops:
@@ -587,7 +564,7 @@ class PlanBuilder:
                 for v in list(op.ins) + [op.res_a, op.res_b]:
                     if v is not None and v.buf is not None and v.bn >= 0:
                         needs.add(v.bn)
-            elif op.kind in (_lib.CONV_BWD_DATA, _lib.CONV_BWD_W, _lib.RES_BWD, _lib.GRAD_COMBINE) and op.out.bn >= 0 \
+            elif op.kind in (_lib.CONV_BWD_DATA, _lib.CONV_BWD_W, _lib.RES_BWD) and op.out.bn >= 0 \
                     and op.out.buf.need_du:
                 needs.add(op.out.bn)
             todo = sorted(b for b in needs if b not in ready)
@@ -688,7 +665,6 @@ def bn_table_struct(plan: Plan):
         s.eps = 1e-5
         s.momentum = 0.1
         s.grad_scale = 1.0 / plan.world
-        s.inline_coef = 1 if getattr(plan, "inline_coef", False) else 0
     return arr
 
 
@@ -735,9 +711,6 @@ def to_c(plan: Plan, ops: List[Op]):
             if bw and ob is not None:
                 c.out.g = _ptr(ob.du) if op.out.bn >= 0 else 0
                 c.out_dxd = _ptr(ob.dxd)
-                if f.combined and op.kind != _lib.GRAD_COMBINE:
-                    # the output gradient was combined in place by GRAD_COMBINE: a plain gradient in `du`
-                    c.out.bn, c.out.g, c.out_dxd = -1, 0, _ptr(ob.du)
         if op.kind == _lib.ZERO:
             t = op.out.buf.du if op.out.bn >= 0 else op.out.buf.dxd
             assert op.out.c0 == 0 and op.out.C == op.out.buf.C, "ZERO clears whole buffers only"

@@ -39,10 +39,6 @@ def op_bytes(op: P.Op) -> int:
             og += 2 * out_b
         elif f.out_act:
             og += out_b
-    if k == _lib.GRAD_COMBINE:
-        return og + out_b                      # read du, x (, dxd), write the combined gradient
-    if f.combined:
-        og = out_b                             # the three backward ops read ONE combined tensor
     if k == _lib.CONV_BWD_W:
         return og + sum(_vbytes(v, N) for v in f.ins)
     if k == _lib.CONV_BWD_DATA:

@@ -163,7 +163,7 @@ def _deps(plan, ops) -> List[Set[int]]:
         elif k == L.STEM_COMPOSE_BWD:
             tr.read(("dWx", f.Wx.off), 0, BIG, i, d)
         else:
-            # BN_FINALIZE_*, GRAD_COMBINE, anything unknown: a full barrier
+            # BN_FINALIZE_*, anything unknown: a full barrier
             d.update(range(i))
             barrier_prev = i
         d.discard(i)

@@ -11,7 +11,6 @@ The per-step host syncs of the reference (`.item()`, barrier; train.py:124-135) 
 from __future__ import annotations
 
 import math
-import os
 from typing import Optional
 
 import torch
@@ -199,12 +198,9 @@ class Trainer:
             self.t_static.copy_(target.reshape(self.t_static.shape), non_blocking=True)
         if self.lr_schedule is not None:
             self.lr_t.fill_(float(self.lr_schedule(self.it)))
-        # world > 1: eager issue by default.  Capturing the NCCL all-reduces into the graph works and measured
-        # 47.0 vs 47.9 ms/step on 2 GPUs, but the processes hung at teardown (graph holding NCCL work destroyed
-        # after the process group) - experimental opt-in SEIST_DDP_GRAPH=1 until that is sorted out.
         # world > 1: with the peer-memory exchange (comm.py) a step contains no NCCL call and is captured like on one
-        # GPU; the NCCL fallback is issued eagerly (capturing NCCL calls hung at teardown, opt-in SEIST_DDP_GRAPH=1)
-        if self.use_graph and (self.world == 1 or self.plan.comm is not None or os.environ.get("SEIST_DDP_GRAPH", "0") == "1"):
+        # GPU; the NCCL fallback is issued eagerly (a graph holding NCCL work hung at teardown)
+        if self.use_graph and (self.world == 1 or self.plan.comm is not None):
             if self.graph is None:
                 before = _lib.lib().seist_launch_count()
                 self._issue()                    # warm-up (also sets kernel attributes)
@@ -214,8 +210,7 @@ class Trainer:
                 # capture on a HIGH-priority stream: the forward/data-gradient chain is the critical path, the
                 # weight-gradient kernels forked onto the engine's default-priority side stream only fill the gaps
                 # (kernel nodes inherit the priority of the stream they were captured from)
-                prio = os.environ.get("SEIST_PRIO", "1") != "0"
-                cap = torch.cuda.Stream(device=self.x_static.device, priority=-1) if prio else None
+                cap = torch.cuda.Stream(device=self.x_static.device, priority=-1)
                 with torch.cuda.graph(g, stream=cap):
                     self._issue()
                 self.graph = g
@@ -223,18 +218,15 @@ class Trainer:
                 self.graph.replay()
         else:
             before = _lib.lib().seist_launch_count()
-            if os.environ.get("SEIST_PRIO", "1") != "0":
-                # same priority split as the captured graph: the step runs on a high-priority stream, the
-                # weight-gradient side stream (default priority) only fills what the main chain leaves idle
-                cur = torch.cuda.current_stream()
-                if getattr(self, "_hp_stream", None) is None:
-                    self._hp_stream = torch.cuda.Stream(device=self.x_static.device, priority=-1)
-                self._hp_stream.wait_stream(cur)
-                with torch.cuda.stream(self._hp_stream):
-                    self._issue()
-                cur.wait_stream(self._hp_stream)
-            else:
+            # same priority split as the captured graph: the step runs on a high-priority stream, the
+            # weight-gradient side stream (default priority) only fills what the main chain leaves idle
+            cur = torch.cuda.current_stream()
+            if getattr(self, "_hp_stream", None) is None:
+                self._hp_stream = torch.cuda.Stream(device=self.x_static.device, priority=-1)
+            self._hp_stream.wait_stream(cur)
+            with torch.cuda.stream(self._hp_stream):
                 self._issue()
+            cur.wait_stream(self._hp_stream)
             self.launches_per_step = int(_lib.lib().seist_launch_count() - before)
         self.it += 1
         return self.loss_out.clone()      # a fresh scalar per step (loss_out itself is overwritten by the next step)

@@ -156,37 +156,6 @@ def test_plan_compiler_vs_oracle_random_cotangent(name, L):
         assert err <= 1e-3 * ref.abs().max().item() + 1e-5 * gmax, (k, err)
 
 
-def test_grad_combine_plan_equals_default_plan(monkeypatch):
-    """GRAD_COMBINE (opt-in, SEIST_COMBINE_CIN): the compiler marks the wide 1x1 convs, emits the in-place BN
-    backward before their three backward ops and re-points those ops at the combined gradient; executed by the
-    interpreter the parameter gradients must equal the default plan's (reference golden batch, train mode)."""
-    g = G.load("seist_s_dpk")
-    x = g["x"][:2, :, :2048].contiguous()
-    tgt = g["target"][:2, :, :2048].contiguous()
-
-    def grads(thr):
-        monkeypatch.setenv("SEIST_COMBINE_CIN", thr)
-        m = create_model("seist_s_dpk", in_channels=3, in_samples=2048)
-        m.load_state_dict(g["state_dict"], strict=True)
-        m.set_drop_rates(**ZERO)
-        flat = P.FlatState(m, torch.device("cpu"))
-        pl = P.PlanBuilder(m, flat, 2, 2048, training=True).build()
-        P.allocate(pl, True)
-        it = Interp(pl)
-        y = it.run_fwd(x).clone()
-        p = y.clone().requires_grad_(True)
-        R.bce_loss(p, tgt).backward()
-        it.run_bwd(p.grad)
-        return pl, flat.G.clone()
-
-    p0, g0 = grads("0")
-    p1, g1 = grads("8")
-    n_comb = sum(op.kind == _lib.GRAD_COMBINE for op in p1.bwd_ops)
-    assert not any(op.kind == _lib.GRAD_COMBINE for op in p0.bwd_ops) and n_comb > 20
-    assert len(p1.bwd_ops) == len(p0.bwd_ops) + n_comb
-    assert (g1 - g0).abs().max().item() <= 1e-5 * g0.abs().max().item()
-
-
 def test_plan_structure_and_sync_points():
     m = create_model("seist_m_dpk", in_channels=3, in_samples=8192)
     flat = P.FlatState(m, torch.device("cpu"))

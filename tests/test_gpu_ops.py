@@ -99,15 +99,6 @@ def test_ops_match_interpreter(name, N, L, training, drops):
     assert _lib.lib().seist_tc_error_flag() == 0, "a tensor-core kernel timed out on an mbarrier"
 
 
-@pytest.mark.gpu
-def test_grad_combine_ops_match_interpreter(monkeypatch):
-    """GRAD_COMBINE (BN backward of the output gradient evaluated once, in place) is opt-in: compile the plans with
-    it enabled for every 1x1 conv of width >= 16 and run the same op-by-op comparison."""
-    monkeypatch.setenv("SEIST_COMBINE_CIN", "16")
-    test_ops_match_interpreter("seist_m_dpk", 2, 2048, True, None)
-    test_ops_match_interpreter("seist_s_dpk", 3, 1000, True, None)      # ragged length: scalar combine path
-
-
 def _run_cases_in_child(env_extra, cases):
     import os
     import subprocess
