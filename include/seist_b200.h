@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 10
+#define SEIST_ABI_VERSION 11
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -200,11 +200,6 @@ int seist_tc_error_flag(void);
 
 /* run ops[0..n) in order on `stream` */
 int seist_plan_run(const SeistOp* ops, int32_t n, void* stream);
-/* same, but the weight-gradient ops (CONV_BWD_W, STEM_COMPOSE_BWD) — which nothing in the backward chain
-   depends on — are issued on `side_stream`, ordered after the preceding ops of `stream` with events and
-   joined back into `stream` before returning (fork/join, CUDA-graph capturable).  side_stream == NULL
-   behaves like seist_plan_run. */
-int seist_plan_run2(const SeistOp* ops, int32_t n, void* stream, void* side_stream);
 
 /* run ops[0..n) on `n_streams` streams by the lane schedule stored in the descriptors: op i is issued on
    streams[min(lane, n_streams-1)] after waiting for its `wait_ev` events; all lanes are forked from streams[0] at the start

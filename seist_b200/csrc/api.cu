@@ -196,7 +196,8 @@ uint64_t seist_launch_count(void) { return seist::g_launches.load(); }
 const char* seist_op_family(const SeistOp* op) { return op ? seist::kFamilyName[seist::choose(*op)] : "none"; }
 int seist_tc_error_flag(void) { return seist::tcconv_error_flag(); }
 
-// fork/join events of seist_plan_run2, one pool per device (events belong to the device that was current at creation)
+// lane and fork/join events of seist_plan_run_lanes, one pool per device (events belong to the device that was current
+// at creation)
 static std::vector<cudaEvent_t> g_events[64];
 static cudaEvent_t event_at(size_t i) {
   int dev = 0;
@@ -211,43 +212,10 @@ static cudaEvent_t event_at(size_t i) {
 }
 static int fork_join(cudaStream_t from, cudaStream_t to, size_t& ev) {
   cudaEvent_t e = event_at(ev++);
-  if (e == nullptr) { seist::set_error("plan_run2: cudaEventCreate failed"); return (int)cudaErrorMemoryAllocation; }
+  if (e == nullptr) { seist::set_error("plan_run_lanes: cudaEventCreate failed"); return (int)cudaErrorMemoryAllocation; }
   cudaError_t r = cudaEventRecord(e, from);
   if (r == cudaSuccess) r = cudaStreamWaitEvent(to, e, 0);
   if (r != cudaSuccess) { seist::set_error(cudaGetErrorString(r)); return (int)r; }
-  return 0;
-}
-
-int seist_plan_run2(const SeistOp* ops, int32_t n, void* stream, void* side_stream) {
-  if (side_stream == nullptr || side_stream == stream) return seist_plan_run(ops, n, stream);
-  if (ops == nullptr || n < 0) { seist::set_error("plan_run2: bad arguments"); return -1; }
-  cudaStream_t s = (cudaStream_t)stream, side = (cudaStream_t)side_stream;
-  size_t ev = 0;
-  bool forked = false, main_dirty = true;
-  for (int i = 0; i < n; ++i) {
-    const bool on_side = ops[i].kind == SEIST_OP_CONV_BWD_W || ops[i].kind == SEIST_OP_STEM_COMPOSE_BWD;
-    int rc;
-    if (on_side) {
-      if (main_dirty) {      // order after everything issued on the main stream so far
-        const int fr = fork_join(s, side, ev);
-        if (fr) return fr;
-        main_dirty = false;
-      }
-      rc = seist::run_one(ops[i], side);
-      forked = true;
-    } else {
-      rc = seist::run_one(ops[i], s);
-      main_dirty = true;
-    }
-    if (rc != 0) {
-      char buf[600];
-      std::snprintf(buf, sizeof(buf), "op %d (kind %d): %s", i, ops[i].kind, seist::g_err);
-      seist::set_error(buf);
-      if (forked) fork_join(side, s, ev);
-      return rc;
-    }
-  }
-  if (forked) return fork_join(side, s, ev);
   return 0;
 }
 

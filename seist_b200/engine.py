@@ -1,5 +1,5 @@
 """Execution engine: owns the flat parameter state and the compiled plans of one model and runs
-them through the C-ABI (`seist_plan_run`) on the current CUDA stream.
+them through the C-ABI (`seist_plan_run_lanes`) from the current CUDA stream.
 
 `Engine.forward` is what `SeismogramTransformer.forward` calls: it is autograd-compatible (the
 returned tensor carries a grad_fn whose backward runs the backward plan and deposits parameter
@@ -10,8 +10,7 @@ consuming kernels (reference training/train.py:374 converts every BN to SyncBatc
 from __future__ import annotations
 
 import ctypes
-import os
-from typing import Dict, Optional, Tuple
+from typing import Dict, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -23,6 +22,14 @@ from . import plan as P
 
 def _stream_ptr() -> int:
     return torch.cuda.current_stream().cuda_stream
+
+
+def run_segment(c_ops, start: int, end: int, streams: Sequence[int]):
+    """Issue the descriptors c_ops[start:end] (one segment of a compiled plan) by their lane schedule on `streams`: the
+    plan's main lanes, then its weight-gradient lane.  Every lane is forked from streams[0] and joined back into it."""
+    arr = (ctypes.c_void_p * len(streams))(*streams)
+    base = ctypes.addressof(c_ops) + start * ctypes.sizeof(_lib.SeistOp)
+    _lib.check(_lib.lib().seist_plan_run_lanes(base, end - start, arr, len(streams)), "seist_plan_run_lanes")
 
 
 class _PlanFn(torch.autograd.Function):
@@ -50,7 +57,6 @@ class Engine:
         self.flat: Optional[P.FlatState] = None
         self.plans: Dict[Tuple, P.Plan] = {}
         self.last_plan: Optional[P.Plan] = None
-        self.overlap_bwd_w = True
         self._side = {}
         self._aux = {}
         self.seed_dev: Optional[torch.Tensor] = None     # ONE dropout step counter (device int64) shared by every plan
@@ -67,6 +73,7 @@ class Engine:
         if self.flat is None or self.flat.device != device or not self.flat.valid():
             self.plans.clear()
             self.flat = P.FlatState(self.model, device)
+            self._named = list(self.model.named_parameters())
             if self.comm is not None:                 # the flat gradient buffer lives in symmetric memory
                 if self.comm.n_grad != self.flat.numel or self.comm.device != device:
                     self.comm = None
@@ -148,42 +155,18 @@ class Engine:
         return pl
 
     # ---- execution -------------------------------------------------------------------------------
-    def _side_stream(self, device) -> int:
-        """Second stream for the weight-gradient ops of the backward plan (fork/join inside plan_run2)."""
-        if not self.overlap_bwd_w:
-            return 0
-        st = self._side.get(device)
-        if st is None:
-            st = self._side[device] = torch.cuda.Stream(device=device)
-        return st.cuda_stream
-
-    def _lane_streams(self, device):
-        """[current stream, aux lane (independent branches), weight-gradient lane] as a ctypes array of stream handles."""
-        from .schedule import n_main_lanes
-        nm = n_main_lanes()
-        aux = self._aux.get(device)
-        if aux is None or len(aux) != nm - 1:
-            aux = self._aux[device] = [torch.cuda.Stream(device=device, priority=-1) for _ in range(nm - 1)]
+    def _lane_streams(self, device, n_main: int):
+        """[current stream, aux lanes (independent branches, high priority), weight-gradient lane (default priority)]"""
+        aux = self._aux.setdefault(device, [])
+        while len(aux) < n_main - 1:
+            aux.append(torch.cuda.Stream(device=device, priority=-1))
         side = self._side.get(device)
         if side is None:
             side = self._side[device] = torch.cuda.Stream(device=device)
-        arr = (ctypes.c_void_p * (nm + 1))(_stream_ptr(), *[a.cuda_stream for a in aux], side.cuda_stream)
-        return arr
+        return [_stream_ptr()] + [a.cuda_stream for a in aux[:n_main - 1]] + [side.cuda_stream]
 
-    def _run_segments(self, plan: P.Plan, c_ops, segs, stat: torch.Tensor, side: bool = False):
-        lib = _lib.lib()
-        base = ctypes.addressof(c_ops)
-        size = ctypes.sizeof(_lib.SeistOp)
-        if (len(segs) == 1 and not segs[0][2] and plan.comm is None and self.overlap_bwd_w
-                and os.environ.get("SEIST_LANES", "1") != "0"):
-            # single GPU: issue the plan over the lanes the scheduler assigned (schedule.py).  Data-parallel plans stay on
-            # one main stream: their BN_PREPARE kernels pair up across ranks by an epoch counter, so every rank must run
-            # them in the same order, which only stream order guarantees.
-            streams = self._lane_streams(plan.device)
-            n = segs[0][1] - segs[0][0]
-            _lib.check(lib.seist_plan_run_lanes(base + segs[0][0] * size, n, streams, len(streams)), "seist_plan_run_lanes")
-            return
-        side_ptr = self._side_stream(plan.device) if side else 0
+    def _run_segments(self, plan: P.Plan, c_ops, segs, stat: torch.Tensor):
+        streams = self._lane_streams(plan.device, plan.n_main)
         for start, end, sync in segs:
             i = 0
             while i < len(sync):          # BN entries registered consecutively own contiguous slots: one call
@@ -193,10 +176,10 @@ class Engine:
                 lo, hi = plan.bns[sync[i]], plan.bns[sync[j]]
                 dist.all_reduce(stat[lo.st_off:hi.st_off + 2 * hi.C])
                 i = j + 1
-            _lib.check(lib.seist_plan_run2(base + start * size, end - start, _stream_ptr(), side_ptr), "seist_plan_run")
+            run_segment(c_ops, start, end, streams)
 
-    def run_forward(self, plan: P.Plan, x: torch.Tensor) -> torch.Tensor:
-        plan.x_in.x.copy_(x)
+    def _issue_forward(self, plan: P.Plan):
+        """The forward plan on the current stream; its input is already in `plan.x_in`."""
         if plan.training:
             # a new set of dropout / DropPath masks for every training forward (the backward of this forward
             # regenerates the same masks from the same counter value)
@@ -207,6 +190,17 @@ class Engine:
         self._run_segments(plan, plan.c_fwd, plan.fwd_segments, plan.stat_acc)
         if plan.training:
             self.flat.NBT[:len(plan.bns)] += 1
+
+    def _issue_backward(self, plan: P.Plan):
+        """The backward plan on the current stream; the output gradient is already in `plan.y_out.dxd`.  It accumulates
+        into the flat gradient buffer, which the caller clears."""
+        plan.gstat_acc.zero_()
+        plan.dWx.zero_()
+        self._run_segments(plan, plan.c_bwd, plan.bwd_segments, plan.gstat_acc)
+
+    def run_forward(self, plan: P.Plan, x: torch.Tensor) -> torch.Tensor:
+        plan.x_in.x.copy_(x)
+        self._issue_forward(plan)
         self.last_plan = plan
         y = plan.y_out.x
         return y if plan.y_out.L > 1 else y[:, :, 0]
@@ -217,11 +211,11 @@ class Engine:
         flat = self.flat
         flat.G.zero_()
         if plan.comm is not None:
+            # no peer is still reading the last backward's partial sums when they are cleared (two backward calls need
+            # not have a forward, and its barrier, in between)
             plan.comm.barrier()
-        plan.gstat_acc.zero_()
-        plan.dWx.zero_()
         plan.y_out.dxd.copy_(dy.reshape(plan.y_out.dxd.shape))
-        self._run_segments(plan, plan.c_bwd, plan.bwd_segments, plan.gstat_acc, side=True)
+        self._issue_backward(plan)
         # one copy of the 1.5 MB buffer: autograd may keep ("steal") the returned tensors as `.grad`, and the flat
         # buffer is zeroed again by the next backward (gradient accumulation over several backward calls must add up)
         out = flat.G.clone()
@@ -236,10 +230,6 @@ class Engine:
         if x.dim() != 3 or x.shape[1] != model.hp.in_channels:
             raise ValueError(f"expected input of shape (N, {model.hp.in_channels}, L), got {tuple(x.shape)}")
         self._ensure_flat(x.device)
-        if not hasattr(self, "_named") or self._named_flat is not self.flat:
-            self._named = list(model.named_parameters())
-            self._name0 = self._named[0][0]
-            self._named_flat = self.flat
         N, _, L = x.shape
         training = model.training
         need_bwd = training and torch.is_grad_enabled()

@@ -149,6 +149,13 @@ class Plan:
         self.fwd_segments: List[Tuple[int, int, List[int]]] = []
         self.bwd_segments: List[Tuple[int, int, List[int]]] = []
 
+    @property
+    def n_main(self) -> int:
+        """Main lanes of the lane schedule (schedule.py), besides the weight-gradient lane.  Data-parallel plans use
+        one: their BN_PREPARE kernels pair up across ranks by an epoch counter, so every rank must issue them in the
+        same order, which one stream guarantees."""
+        return 2 if self.world == 1 else 1
+
 
 class FlatState:
     """One contiguous fp32 buffer for all parameters (+ one for grads, one for BN running stats,
@@ -680,7 +687,7 @@ def _cview(v: Optional[View], use_grad: bool) -> _lib.SeistView:
     return s
 
 
-def to_c(plan: Plan, ops: List[Op]):
+def to_c(plan: Plan, ops: List[Op], segs: List[Tuple[int, int, List[int]]]):
     flat = plan.flat
     arr = (_lib.SeistOp * max(len(ops), 1))()
     for i, op in enumerate(ops):
@@ -743,9 +750,13 @@ def to_c(plan: Plan, ops: List[Op]):
             c.n_bn, c.bn_lo = op.n_bn, op.bn_lo
             if plan.comm is not None and op.sync_bn:
                 c.comm = plan.comm.dev_ptr          # statistic sum over NVLink peer memory fused into this kernel
+    # lane / event fields, one schedule per segment: seist_plan_run_lanes issues a segment per call and joins all lanes at
+    # its end, so event ids are local to the segment
     from .schedule import schedule_lanes
-    info = schedule_lanes(plan, ops, arr)           # lane / event fields (used by seist_plan_run_lanes only)
-    plan.lane_info = getattr(plan, "lane_info", []) + [info]
+    size = ctypes.sizeof(_lib.SeistOp)
+    for start, end, _ in segs:
+        view = (_lib.SeistOp * (end - start)).from_address(ctypes.addressof(arr) + start * size)
+        schedule_lanes(plan, ops[start:end], view, plan.n_main)
     return arr
 
 
@@ -771,9 +782,9 @@ def finalize(plan: Plan, with_backward: bool, step_seed: Optional[torch.Tensor] 
     raw = np.frombuffer(bytes(tab), dtype=np.uint8).copy()
     plan.bn_table_host = tab
     plan.bn_table_dev = torch.from_numpy(raw).to(plan.device)
-    plan.c_fwd = to_c(plan, plan.fwd_ops)
     plan.fwd_segments = segments(plan.fwd_ops, fused=comm is not None)
+    plan.c_fwd = to_c(plan, plan.fwd_ops, plan.fwd_segments)
     if with_backward:
-        plan.c_bwd = to_c(plan, plan.bwd_ops)
         plan.bwd_segments = segments(plan.bwd_ops, fused=comm is not None)
+        plan.c_bwd = to_c(plan, plan.bwd_ops, plan.bwd_segments)
     return plan

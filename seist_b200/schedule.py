@@ -7,12 +7,11 @@ of `MultiPathTransformerLayer` (:396-504), q / k / v projections, the three `DSC
 `schedule_lanes` derives the dependences from the operands' buffers (x / du / dxd slices, BatchNorm statistic slots and
 coefficient tables, composed-weight scratch) and assigns every op a lane; the C executor (`seist_plan_run_lanes`)
 issues each op on its lane's stream and connects the lanes with events, which a CUDA-graph capture turns into graph edges.
-Lane 0 = critical chain (high priority), lane 1 = independent branches, last lane = weight gradients (never on the
-critical path; what `seist_plan_run2` did before).
+Lane 0 = critical chain (high priority), lanes 1 .. n_main - 1 = independent branches, last lane = weight gradients
+(never on the critical path).
 """
 from __future__ import annotations
 
-import os
 from typing import Dict, List, Optional, Set, Tuple
 
 from . import _lib
@@ -181,16 +180,10 @@ def _cost(op) -> float:
     return float(n) * max(1, f.k) ** 0.5 + 2000.0
 
 
-def n_main_lanes() -> int:
-    """main lanes (critical chain + independent branches); SEIST_NMAIN=1..3, default 2"""
-    return min(3, max(1, int(os.environ.get("SEIST_NMAIN", "2"))))
-
-
-def schedule_lanes(plan, ops, c_ops, n_main: Optional[int] = None, cost=_cost) -> dict:
-    """Fill `lane`, `n_wait`, `wait_ev`, `rec_event` of the ctypes descriptors `c_ops`.  Returns a small summary."""
+def schedule_lanes(plan, ops, c_ops, n_main: int, cost=_cost) -> dict:
+    """Fill `lane`, `n_wait`, `wait_ev`, `rec_event` of the ctypes descriptors `c_ops` for `n_main` main lanes (critical
+    chain + independent branches) plus the weight-gradient lane.  Returns a small summary."""
     L = _lib
-    if n_main is None:
-        n_main = n_main_lanes()
     deps = _deps(plan, ops)
     w_lane = n_main                                     # weight-gradient lane
     lane_of: List[int] = []
@@ -204,11 +197,10 @@ def schedule_lanes(plan, ops, c_ops, n_main: Optional[int] = None, cost=_cost) -
     # tail of the step: nothing else is left to overlap with, so they are spread over all lanes instead of queueing on one
     main_kinds = (L.CONV_BWD_DATA, L.RES_BWD, L.ATT_BWD_Q, L.ATT_BWD_KV, L.HEADVEC_BWD, L.CONV_FWD, L.ATT_FWD, L.HEADVEC_FWD)
     last_main = max((i for i, op in enumerate(ops) if op.kind in main_kinds), default=len(ops))
-    spread_tail = os.environ.get("SEIST_TAIL_SPREAD", "1") != "0"
     rr = 0
     for i, op in enumerate(ops):
         d = deps[i]
-        if op.kind == L.CONV_BWD_W and spread_tail and i > last_main:
+        if op.kind == L.CONV_BWD_W and i > last_main:
             lane = (w_lane + rr) % (n_main + 1)
             rr += 1
         elif op.kind in (L.CONV_BWD_W, L.STEM_COMPOSE_BWD):

@@ -65,10 +65,6 @@ class Trainer:
         eng = m.engine()
         dev = x.device
         eng._ensure_flat(dev)
-        if not hasattr(eng, "_named") or eng._named_flat is not eng.flat:
-            eng._named = list(m.named_parameters())
-            eng._name0 = eng._named[0][0]
-            eng._named_flat = eng.flat
         m.train()
         N, _, L = x.shape
         self.plan = eng.get_plan(N, L, True, True)
@@ -112,13 +108,7 @@ class Trainer:
         lib = _lib.lib()
         plan, eng, flat = self.plan, self.eng, self.flat
         s = torch.cuda.current_stream().cuda_stream
-        _lib.check(lib.seist_advance_seed(plan.step_seed.data_ptr(), s))
-        comm = plan.comm
-        if comm is not None:
-            comm.barrier()               # every peer has finished reading last step's partial statistics / gradients
-        plan.stat_acc.zero_()
-        eng._run_segments(plan, plan.c_fwd, plan.fwd_segments, plan.stat_acc)
-        flat.NBT[:len(plan.bns)] += 1
+        eng._issue_forward(plan)         # its barrier: every peer has finished reading last step's statistics / gradients
         y, dy, t = plan.y_out.x, plan.y_out.dxd, self.t_static
         if isinstance(self.loss_fn, BCELoss):
             N, C, L = y.shape
@@ -133,14 +123,12 @@ class Trainer:
             _lib.check(lib.seist_huber_bwd(y.data_ptr(), t.data_ptr(), self.gout.data_ptr(), y.numel(),
                                            self.loss_fn.delta, dy.data_ptr(), s))
         flat.G.zero_()
-        plan.gstat_acc.zero_()
-        plan.dWx.zero_()
-        eng._run_segments(plan, plan.c_bwd, plan.bwd_segments, plan.gstat_acc, side=True)
+        eng._issue_backward(plan)
         gscale = 1.0
         grads = flat.G
         if self.world > 1:
-            if comm is not None:
-                grads = comm.allreduce_grads()   # one kernel reading every peer's 1.5 MB over NVLink (C1), no NCCL
+            if plan.comm is not None:
+                grads = plan.comm.allreduce_grads()   # one kernel reading every peer's 1.5 MB over NVLink (C1), no NCCL
             else:
                 dist.all_reduce(flat.G)          # NCCL fallback (SEIST_SYMM=0 / plain BatchNorm)
             gscale = 1.0 / self.world

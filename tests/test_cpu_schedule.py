@@ -38,10 +38,9 @@ def _happens_before_ok(ops, c_ops, deps, n_lanes):
 
 
 @pytest.mark.parametrize("n_main", [1, 2, 3])
-@pytest.mark.parametrize("tail", ["0", "1"])
-def test_lane_schedule_covers_every_dependence(n_main, tail, monkeypatch):
-    monkeypatch.setenv("SEIST_TAIL_SPREAD", tail)
-    m = create_model("seist_s_dpk", in_channels=3, in_samples=2048)
+@pytest.mark.parametrize("name", ["seist_s_dpk", "seist_m_dpk"])
+def test_lane_schedule_covers_every_dependence(name, n_main):
+    m = create_model(name, in_channels=3, in_samples=2048)
     flat = P.FlatState(m, torch.device("cpu"))
     pl = P.PlanBuilder(m, flat, 2, 2048, training=True).build()
     for ops in (pl.fwd_ops, pl.bwd_ops):
@@ -59,12 +58,33 @@ def test_lane_schedule_covers_every_dependence(n_main, tail, monkeypatch):
     main_kinds = (L.CONV_BWD_DATA, L.RES_BWD, L.ATT_BWD_Q, L.ATT_BWD_KV, L.HEADVEC_BWD)
     last_main = max(i for i, o in enumerate(ops) if o.kind in main_kinds)
     for i, o in enumerate(ops):
-        if o.kind == L.CONV_BWD_W and (i < last_main or tail == "0"):
+        if o.kind == L.CONV_BWD_W and i < last_main:
             assert c_ops[i].lane == n_main
 
 
-def test_default_lane_count(monkeypatch):
-    monkeypatch.delenv("SEIST_NMAIN", raising=False)
-    assert schedule.n_main_lanes() == 2
-    monkeypatch.setenv("SEIST_NMAIN", "7")
-    assert schedule.n_main_lanes() == 3
+def test_plan_lane_count():
+    m = create_model("seist_s_dpk", in_channels=3, in_samples=1024)
+    flat = P.FlatState(m, torch.device("cpu"))
+    assert P.PlanBuilder(m, flat, 2, 1024, training=True, world=1).build().n_main == 2
+    assert P.PlanBuilder(m, flat, 2, 1024, training=True, world=2).build().n_main == 1
+
+
+def test_data_parallel_plan_is_scheduled_per_segment_on_one_main_lane():
+    """world = 2 without the peer-memory exchange: the plan is cut into segments with a statistic all-reduce between
+    them, and seist_plan_run_lanes issues one segment per call, so each segment's schedule must stand on its own.  One
+    main lane keeps every BN_PREPARE in plan order on every rank."""
+    m = create_model("seist_s_dpk", in_channels=3, in_samples=2048)
+    flat = P.FlatState(m, torch.device("cpu"))
+    pl = P.finalize(P.PlanBuilder(m, flat, 2, 2048, training=True, world=2).build(), True)
+    assert pl.n_main == 1
+    for ops, c_ops, segs in ((pl.fwd_ops, pl.c_fwd, pl.fwd_segments), (pl.bwd_ops, pl.c_bwd, pl.bwd_segments)):
+        assert len(segs) > 1
+        for start, end, _ in segs:
+            seg_ops, seg_c = ops[start:end], c_ops[start:end]
+            assert _happens_before_ok(seg_ops, seg_c, schedule._deps(pl, seg_ops), pl.n_main + 1)
+            n = end - start
+            for c in seg_c:
+                assert -1 <= c.rec_event < n
+                assert all(0 <= c.wait_ev[q] < n for q in range(c.n_wait))
+                if c.kind not in (_lib.CONV_BWD_W, _lib.STEM_COMPOSE_BWD):
+                    assert c.lane == 0

@@ -22,6 +22,7 @@ from harness import ZERO_DROPS, randomize
 from oracle import seist_ref as R
 from seist_b200 import _lib
 from seist_b200 import plan as P
+from seist_b200.engine import run_segment
 from seist_b200.models import create_model
 from seist_b200.models.loss import BCELoss
 
@@ -209,19 +210,25 @@ def test_dropout_advances_per_forward_and_follows_manual_seed():
 # ------------------------------------------------------------------------------------------------
 # SyncBatchNorm data parallelism on one GPU ("virtual world 2")
 # ------------------------------------------------------------------------------------------------
+def _extra_lanes(plan):
+    """one stream for every lane of the plan's schedule after the first (the caller supplies lane 0)"""
+    return [torch.cuda.Stream() for _ in range(plan.n_main)]
+
+
 def _run_segments_lockstep(plans, which, reduce_slices):
-    lib = _lib.lib()
-    size = ctypes.sizeof(_lib.SeistOp)
+    """Issue segment j of every rank's plan, then segment j + 1, ...  Every rank runs its lane schedule from the current
+    stream on lanes of its own; `reduce_slices` sums the statistics on the current stream before a segment needs them."""
     s = torch.cuda.current_stream().cuda_stream
+    extra = [_extra_lanes(p) for p in plans]
     segs = [getattr(p, which + "_segments") for p in plans]
     assert all(len(sg) == len(segs[0]) for sg in segs)
     for j in range(len(segs[0])):
         start, end, sync = segs[0][j]
         if sync:
             reduce_slices(sync)
-        for p in plans:
+        for p, ex in zip(plans, extra):
             c_ops = p.c_fwd if which == "fwd" else p.c_bwd
-            _lib.check(lib.seist_plan_run(ctypes.addressof(c_ops) + start * size, end - start, s), which)
+            run_segment(c_ops, start, end, [s] + [e.cuda_stream for e in ex])
     torch.cuda.synchronize()
 
 
@@ -471,13 +478,12 @@ def test_fused_peer_exchange_two_virtual_ranks_equal_single_rank():
     s0 = torch.cuda.current_stream().cuda_stream
     p1.x_in.x.copy_(x)
     p1.stat_acc.zero_()
-    _lib.check(lib.seist_plan_run(ctypes.addressof(p1.c_fwd), len(p1.fwd_ops), s0))
+    _run_segments_lockstep([p1], "fwd", lambda sync: None)
     y = p1.y_out.x
     gout = torch.ones(1, device="cuda")
     _lib.check(lib.seist_bce_bwd(y.data_ptr(), t.data_ptr(), w.data_ptr(), gout.data_ptr(), NB, 3, L, 1e-6, p1.y_out.dxd.data_ptr(), s0))
     f1.G.zero_(); p1.gstat_acc.zero_(); p1.dWx.zero_()
-    _lib.check(lib.seist_plan_run(ctypes.addressof(p1.c_bwd), len(p1.bwd_ops), s0))
-    torch.cuda.synchronize()
+    _run_segments_lockstep([p1], "bwd", lambda sync: None)
 
     # two virtual ranks
     ranks = [model_and_flat() for _ in range(W)]
@@ -496,6 +502,7 @@ def test_fused_peer_exchange_two_virtual_ranks_equal_single_rank():
              for r, (m, f) in enumerate(ranks)]
     assert any(op.kind == _lib.BN_PREPARE_FWD and op.sync_bn for op in plans[0].fwd_ops)
     streams = [torch.cuda.Stream() for _ in range(W)]
+    extra = [_extra_lanes(p) for p in plans]
     n = NB // W
     gos = [torch.ones(1, device="cuda") for _ in range(W)]
     tts = [t[r * n:(r + 1) * n].contiguous() for r in range(W)]
@@ -510,18 +517,25 @@ def test_fused_peer_exchange_two_virtual_ranks_equal_single_rank():
         for st in streams:
             st.synchronize()
 
+    def issue(r, pl, which, s):
+        """rank r's plan by its lane schedule: lane 0 on the rank's stream, the other lanes on streams of its own"""
+        c_ops = pl.c_fwd if which == "fwd" else pl.c_bwd
+        for start, end, sync in getattr(pl, which + "_segments"):
+            assert not sync          # the statistic exchange is inside the BN_PREPARE kernels
+            run_segment(c_ops, start, end, [s] + [e.cuda_stream for e in extra[r]])
+
     def p_fwd(r, pl, cm, fl, s):
         pl.x_in.x.copy_(x[r * n:(r + 1) * n])
         cm.barrier(stream=s)
         pl.stat_acc.zero_()
-        _lib.check(lib.seist_plan_run(ctypes.addressof(pl.c_fwd), len(pl.fwd_ops), s))
+        issue(r, pl, "fwd", s)
 
     def p_bwd(r, pl, cm, fl, s):
         yy = pl.y_out.x        # local-mean loss, like every rank of the real job (1/world is applied to the reduced sum)
         _lib.check(lib.seist_bce_bwd(yy.data_ptr(), tts[r].data_ptr(), w.data_ptr(), gos[r].data_ptr(), n, 3, L, 1e-6,
                                      pl.y_out.dxd.data_ptr(), s))
         fl.G.zero_(); pl.gstat_acc.zero_(); pl.dWx.zero_()
-        _lib.check(lib.seist_plan_run(ctypes.addressof(pl.c_bwd), len(pl.bwd_ops), s))
+        issue(r, pl, "bwd", s)
 
     def p_red(r, pl, cm, fl, s):
         cm.allreduce_grads(stream=s)
