@@ -40,6 +40,8 @@ int launch_bn_finalize(const SeistOp& op, bool fwd, cudaStream_t s);
 bool pw_eligible(const SeistOp& op);
 int launch_pw_fwd(const SeistOp& op, cudaStream_t s, int sm_count);
 int launch_pw_bwd_data(const SeistOp& op, cudaStream_t s, int sm_count);
+bool pw_bwd_data_staged_ok(const SeistOp& op);
+int launch_pw_bwd_data_staged(const SeistOp& op, cudaStream_t s, int sm_count);
 int launch_res_bwd4(const SeistOp& op, cudaStream_t s, int sm_count);
 bool bww_eligible(const SeistOp& op);
 int launch_bww_any(const SeistOp& op, cudaStream_t s, int sm_count);
@@ -100,14 +102,14 @@ static int validate_conv(const SeistOp& op) {
 
 // which kernel family serves an op (also reported to the bench: `seist_op_family`)
 enum Family {
-  F_NONE = 0, F_TCCONV_FWD, F_TCCONV_BWD_DATA, F_PW_FWD, F_CONVK_FWD, F_CONV_FWD, F_PW_BWD_DATA, F_CONVK_BWD_DATA,
+  F_NONE = 0, F_TCCONV_FWD, F_TCCONV_BWD_DATA, F_PW_FWD, F_CONVK_FWD, F_CONV_FWD, F_PW_BWD_DATA, F_PW_BWD_DATA_STAGED, F_CONVK_BWD_DATA,
   F_CONV_BWD_DATA, F_BWWK, F_BWW, F_CONV_BWD_W, F_RES_BWD, F_RES_BWD4, F_ATT_FWD, F_ATT_BWD_Q, F_ATT_BWD_KV, F_HEADVEC_FWD,
   F_HEADVEC_BWD, F_BN_FINALIZE_FWD, F_BN_FINALIZE_BWD, F_BN_PREPARE_FWD, F_BN_PREPARE_BWD, F_STEM_COMPOSE_FWD, F_STEM_COMPOSE_BWD,
   F_ZERO
 };
 static const char* kFamilyName[] = {
   "none", "tcconv_fwd(wgmma+TMA)", "tcconv_bwd_data(wgmma+TMA)", "pw_fwd(simt)", "convk_fwd(simt)",
-  "conv_fwd(simt)", "pw_bwd_data(simt)", "convk_bwd_data(simt)", "conv_bwd_data(simt)", "bwwk(simt)", "bww(simt)",
+  "conv_fwd(simt)", "pw_bwd_data(simt)", "pw_bwd_data_staged(simt)", "convk_bwd_data(simt)", "conv_bwd_data(simt)", "bwwk(simt)", "bww(simt)",
   "conv_bwd_w(simt)", "res_bwd", "res_bwd4", "att_fwd", "att_bwd_q", "att_bwd_kv", "headvec_fwd", "headvec_bwd", "bn_finalize_fwd",
   "bn_finalize_bwd", "bn_prepare_fwd", "bn_prepare_bwd", "stem_compose_fwd", "stem_compose_bwd", "zero"
 };
@@ -120,6 +122,7 @@ static Family choose(const SeistOp& op) {
       return convk_eligible(op) ? F_CONVK_FWD : F_CONV_FWD;
     case SEIST_OP_CONV_BWD_DATA:
       if (use_tcc(op, 1)) return F_TCCONV_BWD_DATA;
+      if (pw_bwd_data_staged_ok(op)) return F_PW_BWD_DATA_STAGED;
       if (pw_eligible(op)) return F_PW_BWD_DATA;
       return convk_bwd_data_eligible(op) ? F_CONVK_BWD_DATA : F_CONV_BWD_DATA;
     case SEIST_OP_CONV_BWD_W:
@@ -154,6 +157,7 @@ static int run_one(const SeistOp& op, cudaStream_t s) {
     case F_CONVK_FWD: return launch_convk_fwd(op, s);
     case F_CONV_FWD: return launch_conv_fwd(op, s);
     case F_PW_BWD_DATA: return launch_pw_bwd_data(op, s, sm_count());
+    case F_PW_BWD_DATA_STAGED: return launch_pw_bwd_data_staged(op, s, sm_count());
     case F_CONVK_BWD_DATA: return launch_convk_bwd_data(op, s);
     case F_CONV_BWD_DATA: return launch_conv_bwd_data(op, s);
     case F_BWWK: return launch_bwwk(op, s, sm_count());

@@ -630,6 +630,254 @@ __global__ void __launch_bounds__(PW_NT, 4) pw_bwd_data_kernel(const __grid_cons
 }
 
 // ================================================================================================
+// backward (data), staged: one CTA owns a tile of 128 samples and ALL target channels of the op, so every output-channel
+// operand (dxd | du | x) is read from memory once and its gradient combine (BN-backward, sigmoid', drop factors, dropout
+// mask) is evaluated once, instead of once per 16-target tile.  Warp w holds targets 16w .. 16w+15 (same 16 x 4 register
+// tile as pw_bwd_data_kernel, lane = quad of 4 samples).  The operands of PWS_CC output channels form one stage of a
+// PWS_S-deep shared-memory ring filled with cp.async; the thread that copied a (channel, quad) slot combines it in place
+// after its own wait_group, then one barrier publishes the stage to every warp.  Persistent grid over sample tiles.
+// blockDim = 32 * ceil(Cin / 16).
+// ================================================================================================
+constexpr int PWS_CC = 8;                          // output channels per ring stage
+constexpr int PWS_S = 3;                           // ring stages (PWS_S - 1 stages in flight while one is consumed)
+constexpr int PWS_PLANE_B = 32 * 16;               // one channel plane of a tile: 32 quads x 16 bytes
+constexpr int PWS_STAGE_B = PWS_CC * 3 * PWS_PLANE_B;   // [channel][dxd | du | x][quad] float4
+constexpr int PWS_MAX_CIN = 192;                   // 12 warps
+
+__device__ __forceinline__ void sts4(uint32_t a, float4 v) {
+  asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
+// one reduce-scatter step: lanes with bit H set keep values [H, 2H), the others [0, H); each adds its partner's half
+template <int H>
+__device__ __forceinline__ void warp_halve(float* v, int lane) {
+  const bool up = (lane & H) != 0;
+#pragma unroll
+  for (int k = 0; k < H; ++k) {
+    const float send = up ? v[k] : v[k + H];
+    const float keep = up ? v[k + H] : v[k];
+    v[k] = keep + __shfl_xor_sync(0xffffffffu, send, H);
+  }
+}
+
+template <bool F_ELEM, bool F_GELU>
+__global__ void __launch_bounds__(PWS_MAX_CIN * 2) pw_bwd_data_staged_kernel(const __grid_constant__ SeistOp op) {
+  extern __shared__ __align__(16) unsigned char sm_raw[];
+  const int NT = blockDim.x, NW = NT >> 5;
+  const int Cout = op.Cout, Cin = op.Cin, Cin16 = NW * 16;
+  const int nck = (Cout + PWS_CC - 1) / PWS_CC, CoutC = nck * PWS_CC;
+  PwChan* ch_s = reinterpret_cast<PwChan*>(sm_raw);                       // [Cin16] targets
+  PwOut* oc_s = reinterpret_cast<PwOut*>(ch_s + Cin16);                   // [CoutC]
+  float* w_s = reinterpret_cast<float*>(oc_s + CoutC);                    // [CoutC][Cin16]
+  const uint32_t ring = smem_addr(w_s + CoutC * Cin16);                   // [PWS_S] stages (16-byte aligned carve-up)
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int L = op.L_out, LQ = L >> 2;
+
+  for (int ci = tid; ci < Cin16; ci += NT) {
+    PwChan c = make_chan(op, ci < Cin ? ci : 0, true);
+    if (ci >= Cin) c.g = nullptr;
+    ch_s[ci] = c;
+  }
+  for (int co = tid; co < CoutC; co += NT) {
+    PwOut o = {0.f, 0.f, 0.f};
+    if (co < Cout) {
+      const OutGradCoef k = out_grad_coef(op, co);
+      o.A = k.A;
+      o.Bx = k.Bx;
+      o.Cc = k.Cc;
+    }
+    oc_s[co] = o;
+  }
+  for (int idx = tid; idx < CoutC * Cin16; idx += NT) {
+    const int co = idx / Cin16, ci = idx - co * Cin16;
+    w_s[idx] = (co < Cout && ci < Cin) ? op.W[(size_t)co * Cin + ci] : 0.f;
+  }
+  __syncthreads();
+
+  const uint64_t seed = load_seed(op.step_seed);
+  const long long NQ = (long long)op.N * LQ;
+  const long long ntiles = (NQ + 31) / 32;
+  const bool has_dxd = op.out_dxd != nullptr;
+  const bool has_bn = (op.out.bn >= 0 && op.out.g != nullptr);
+  const bool need_x = has_bn || op.out_act == SEIST_OUT_SIGMOID;
+  auto quad_of = [&](long long tile, int& n, int& l) -> bool {
+    const long long f = tile * 32 + lane;
+    const bool ok = f < NQ;
+    n = ok ? (int)(f / LQ) : 0;
+    l = ok ? (int)(f - (long long)n * LQ) * 4 : 0;
+    return ok;
+  };
+
+  // issue cursor over the flattened (tile, channel chunk) sequence, PWS_S - 1 stages ahead of the consumer; a thread
+  // copies channels warp, warp + NW, ... of a chunk at quad `lane` (and later combines exactly those slots)
+  long long itile = blockIdx.x;
+  int ick = 0, istage = 0;
+  int in_, il;
+  bool iok = quad_of(itile, in_, il);
+  size_t iobase = ((size_t)in_ * op.out.Ct + op.out.c0) * (size_t)L + il;
+  auto issue_step = [&]() {
+    if (itile < ntiles) {
+      const uint32_t dst0 = ring + istage * PWS_STAGE_B + lane * 16;
+      for (int c = warp; c < PWS_CC; c += NW) {
+        const int co = ick * PWS_CC + c;
+        if (iok && co < Cout) {
+          const size_t off = iobase + (size_t)co * L;
+          const uint32_t dst = dst0 + c * (3 * PWS_PLANE_B);
+          if (has_dxd) cp_async16(dst, op.out_dxd + off);
+          if (has_bn) cp_async16(dst + PWS_PLANE_B, op.out.g + off);
+          if (need_x) cp_async16(dst + 2 * PWS_PLANE_B, op.out.x + off);
+        }
+      }
+      if (++ick == nck) {
+        ick = 0;
+        itile += gridDim.x;
+        iok = quad_of(itile, in_, il);
+        iobase = ((size_t)in_ * op.out.Ct + op.out.c0) * (size_t)L + il;
+      }
+    }
+    cp_async_commit();   // one group per step (possibly empty) keeps the wait count uniform
+    istage = istage + 1 == PWS_S ? 0 : istage + 1;
+  };
+#pragma unroll
+  for (int s = 0; s < PWS_S - 1; ++s) issue_step();
+
+  bool warp_bn = false;   // any BN-backward target in this warp (warp-uniform)
+  for (int t = 0; t < 16; ++t) {
+    const PwChan& c = ch_s[warp * 16 + t];
+    warp_bn |= c.g != nullptr && c.bn >= 0;
+  }
+  const PwChan* my_ch = ch_s + warp * 16;
+  float st_run = 0.f;   // lane i: BN-backward sum (i & 1) of target warp * 16 + (i >> 1), over this CTA's tiles
+  int cstage = 0;
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int n, l;
+    const bool ok = quad_of(tile, n, l);
+    const float pf = path_factor(op, seed, n) * alpha_factor(op, seed, n);
+    float2 acc[8][4];   // [target pair][sample] (fma2 lanes = even / odd target)
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[c][q] = make_float2(0.f, 0.f);
+    for (int ck = 0; ck < nck; ++ck) {
+      cp_async_wait<PWS_S - 2>();
+      const uint32_t st = ring + cstage * PWS_STAGE_B + lane * 16;
+      cstage = cstage + 1 == PWS_S ? 0 : cstage + 1;
+      for (int c = warp; c < PWS_CC; c += NW) {
+        const int co = ck * PWS_CC + c;
+        const uint32_t slot = st + c * (3 * PWS_PLANE_B);
+        float4 gv = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (ok && co < Cout) {
+          const float4 dx = has_dxd ? lds4(slot) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 du = has_bn ? lds4(slot + PWS_PLANE_B) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 xo = need_x ? lds4(slot + 2 * PWS_PLANE_B) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const PwOut o = oc_s[co];
+          gv.x = dx.x + fmaf(o.A, du.x, fmaf(o.Bx, xo.x, o.Cc));
+          gv.y = dx.y + fmaf(o.A, du.y, fmaf(o.Bx, xo.y, o.Cc));
+          gv.z = dx.z + fmaf(o.A, du.z, fmaf(o.Bx, xo.z, o.Cc));
+          gv.w = dx.w + fmaf(o.A, du.w, fmaf(o.Bx, xo.w, o.Cc));
+          if (op.out_act == SEIST_OUT_SIGMOID) {
+            gv.x *= xo.x * (1.f - xo.x);
+            gv.y *= xo.y * (1.f - xo.y);
+            gv.z *= xo.z * (1.f - xo.z);
+            gv.w *= xo.w * (1.f - xo.w);
+          }
+          gv.x *= pf;
+          gv.y *= pf;
+          gv.z *= pf;
+          gv.w *= pf;
+          if (F_ELEM) {
+            const float4 kp = pw_keep4(op.p_elem, seed, op.seed_elem, ((uint64_t)n * Cout + co) * (uint64_t)L + l);
+            gv.x *= kp.x;
+            gv.y *= kp.y;
+            gv.z *= kp.z;
+            gv.w *= kp.w;
+          }
+        }
+        sts4(slot, gv);   // channels past Cout / quads past the end contribute zeros
+      }
+      __syncthreads();
+      issue_step();       // refills the slot every warp finished reading before the barrier
+      const float* wr0 = w_s + ck * PWS_CC * Cin16 + warp * 16;
+#pragma unroll
+      for (int c = 0; c < PWS_CC; ++c) {
+        const float4 g = lds4(st + c * (3 * PWS_PLANE_B));
+        const float2* wr = reinterpret_cast<const float2*>(wr0 + c * Cin16);
+        const float2 gx = dup2(g.x), gy = dup2(g.y), gz = dup2(g.z), gw = dup2(g.w);
+#pragma unroll
+        for (int cp = 0; cp < 8; ++cp) {
+          const float2 w = wr[cp];
+          acc[cp][0] = fma2(w, gx, acc[cp][0]);
+          acc[cp][1] = fma2(w, gy, acc[cp][1]);
+          acc[cp][2] = fma2(w, gz, acc[cp][2]);
+          acc[cp][3] = fma2(w, gw, acc[cp][3]);
+        }
+      }
+    }
+    // epilogue of this warp's targets, in batches of PW_BD_EB channels (all loads of a batch before its first store)
+    float bs[32];   // [2 * target + k]: BN-backward sums of this quad
+#pragma unroll
+    for (int cb = 0; cb < 16; cb += PW_BD_EB) {
+      float4 xv[PW_BD_EB], ov[PW_BD_EB];
+#pragma unroll
+      for (int u = 0; u < PW_BD_EB; ++u) {
+        const PwChan& c = my_ch[cb + u];
+        const long long off = (long long)n * c.nstride + l;
+        const bool live = ok && c.g != nullptr;
+        const bool want_x = live && ((F_GELU && c.act == SEIST_ACT_GELU) || c.bn >= 0);
+        xv[u] = want_x ? ldg4(c.x + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+        ov[u] = (live && c.accum) ? ld4(c.g + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+#pragma unroll
+      for (int u = 0; u < PW_BD_EB; ++u) {
+        const int col = cb + u;
+        const PwChan& c = my_ch[col];
+        bs[2 * col] = 0.f;
+        bs[2 * col + 1] = 0.f;
+        if (!ok || c.g == nullptr) continue;
+        const float2(&ap)[4] = acc[col >> 1];
+        float4 gg = (col & 1) ? make_float4(ap[0].y, ap[1].y, ap[2].y, ap[3].y) : make_float4(ap[0].x, ap[1].x, ap[2].x, ap[3].x);
+        const float4 x = xv[u];
+        if (F_GELU && c.act == SEIST_ACT_GELU) {
+          const float4 d = pw_gelu_grad4(make_float4(fmaf(c.sc, x.x, c.sh), fmaf(c.sc, x.y, c.sh), fmaf(c.sc, x.z, c.sh),
+                                                     fmaf(c.sc, x.w, c.sh)));
+          gg.x *= d.x;
+          gg.y *= d.y;
+          gg.z *= d.z;
+          gg.w *= d.w;
+        }
+        if (c.bn >= 0) {
+          bs[2 * col] = (gg.x + gg.y) + (gg.z + gg.w);
+          bs[2 * col + 1] = fmaf(gg.x, (x.x - c.mu) * c.istd, gg.y * ((x.y - c.mu) * c.istd)) +
+                            fmaf(gg.z, (x.z - c.mu) * c.istd, gg.w * ((x.w - c.mu) * c.istd));
+        }
+        gg.x += ov[u].x;
+        gg.y += ov[u].y;
+        gg.z += ov[u].z;
+        gg.w += ov[u].w;
+        st4(c.g + (long long)n * c.nstride + l, gg);
+      }
+    }
+    if (warp_bn) {
+      // reduce-scatter over the warp (31 shuffles): afterwards bs[0] of lane i is the warp's sum of value i
+      warp_halve<16>(bs, lane);
+      warp_halve<8>(bs, lane);
+      warp_halve<4>(bs, lane);
+      warp_halve<2>(bs, lane);
+      warp_halve<1>(bs, lane);
+      st_run += bs[0];
+    }
+  }
+  cp_async_wait<0>();
+  if (warp_bn) {
+    const PwChan& c = my_ch[lane >> 1];
+    if (c.g != nullptr && c.bn >= 0) {
+      const SeistBN& e = op.bn_table[c.bn];
+      atomicAdd(&e.gstat_acc[(lane & 1) * e.C + c.bnc], (double)st_run);
+    }
+  }
+}
+
+// ================================================================================================
 // backward: residual pass-through, vectorised.  grid (ceil(NQ/(128*G)), Cout): one channel per CTA.
 // ================================================================================================
 __global__ void __launch_bounds__(PW_NT) res_bwd4_kernel(const __grid_constant__ SeistOp op, const int G) {
@@ -820,6 +1068,54 @@ int launch_pw_bwd_data(const SeistOp& op, cudaStream_t s, int sm_count) {
   if (rc) return rc;
   note_launch();
   return check_launch("pw_bwd_data");
+}
+
+static size_t pw_bwd_data_staged_smem(const SeistOp& op) {
+  const int cin16 = (op.Cin + 15) & ~15, coutc = (op.Cout + PWS_CC - 1) / PWS_CC * PWS_CC;
+  return sizeof(PwChan) * cin16 + sizeof(PwOut) * coutc + sizeof(float) * (size_t)coutc * cin16 + (size_t)PWS_S * PWS_STAGE_B;
+}
+
+// Non-pooled 1x1 data gradients with more than one 16-target tile, whose weights and ring fit one CTA's shared memory.
+// Two-tile ops (Cin <= 32) with a GELU target stay on pw_bwd_data_kernel: there the staged CTA is two warps whose GELU'
+// epilogue is not hidden behind the ring, and it measured slower on H100 than reading the operands twice.
+bool pw_bwd_data_staged_ok(const SeistOp& op) {
+  return pw_eligible(op) && op.pool <= 1 && op.Cin > 16 && op.Cin <= PWS_MAX_CIN && (op.Cin > 32 || !any_gelu(op)) &&
+         pw_bwd_data_staged_smem(op) <= 227 * 1024;
+}
+
+template <bool E, bool Gf>
+static int pw_bwdd_staged_go(const SeistOp& op, cudaStream_t s, int sm_count) {
+  const auto kernel = pw_bwd_data_staged_kernel<E, Gf>;
+  const size_t smem = pw_bwd_data_staged_smem(op);
+  const int nt = 32 * ((op.Cin + 15) / 16);
+  int rc = pw_set_smem(kernel, smem);
+  if (rc) return rc;
+  int per_sm = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, nt, smem);
+  if (e != cudaSuccess) return (int)e;
+  if (per_sm < 1) {
+    set_error("pw_bwd_data_staged: no resident CTA fits");
+    return -2;
+  }
+  const long long tiles = ((long long)op.N * (op.L_out >> 2) + 31) / 32;
+  const long long resident = (long long)per_sm * sm_count;
+  const long long grid = tiles < resident ? tiles : resident;
+  kernel<<<(unsigned)grid, nt, smem, s>>>(op);
+  return 0;
+}
+
+int launch_pw_bwd_data_staged(const SeistOp& op, cudaStream_t s, int sm_count) {
+  const int sel = (op.p_elem > 0.f ? 2 : 0) | (any_gelu(op) ? 1 : 0);
+  int rc;
+  switch (sel) {
+    case 0: rc = pw_bwdd_staged_go<false, false>(op, s, sm_count); break;
+    case 1: rc = pw_bwdd_staged_go<false, true>(op, s, sm_count); break;
+    case 2: rc = pw_bwdd_staged_go<true, false>(op, s, sm_count); break;
+    default: rc = pw_bwdd_staged_go<true, true>(op, s, sm_count); break;
+  }
+  if (rc) return rc;
+  note_launch();
+  return check_launch("pw_bwd_data_staged");
 }
 
 int launch_res_bwd4(const SeistOp& op, cudaStream_t s, int sm_count) {
