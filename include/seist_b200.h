@@ -262,10 +262,36 @@ int seist_det_counters(const int64_t* targets, const int64_t* preds, int64_t N, 
                       then mode 1 "std" / 2 "max" scaling (a zero scale is replaced by 1), mode 0 "" mean removal only.
    seist_dpk_labels = the label stack [det, ppk, spk] of the dpk task (config.py:137-146) from the phase indices:
                       _generate_soft_label (:544-683) with _pad_phases (:16-35).  ppks / spks: (N, K) int64, entries
-                      <= -1000000 mean "no phase"; shape 0 gaussian (sigma 10 samples) / 1 triangle / 2 box; out (N,3,L). */
+                      <= -1000000 mean "no phase"; shape 0 gaussian (sigma 10 samples) / 1 triangle / 2 box /
+                      3 sigmoid (width >= 2); out (N,3,L). */
 int seist_normalize(float* x, int64_t rows, int32_t L, int32_t mode, void* stream);
 int seist_dpk_labels(const int64_t* ppks, const int64_t* spks, int64_t N, int32_t K, int32_t L, int32_t width,
                      int32_t shape, double coda_ratio, float* out, void* stream);
+
+/* ---- training-time augmentation on the device (reference training/preprocess.py) ---------------------------------
+   seist_augment = DataPreprocessor.process (:501-542) for a batch: _is_noise, _pad_phases, _data_augmentation (:432-499)
+                   where augment[n] != 0 (every trace when augment is NULL), _cut_window (:172-222), _normalize.
+                   data (N, C, Lin) fp32, 3 <= Lin <= 16384 and C * Lin * 4 bytes within the shared memory of one CTA;
+                   ppks / spks (N, K) int64, entries <= -1000000 mean "no phase"; snr (N, S) double or S = 0.
+                   Writes x (N, C, cfg->in_samples), the output phase lists ppks_out / spks_out (N, K_out) padded with
+                   -10000000, cleared (N,) (1 where _is_noise or the generated noise cleared the event).  Draws come from a
+                   counter-based generator at *seed (device scalar, not advanced here).  work: N * seist_aug_recipe_bytes().
+   seist_sizeof_aug = sizeof(SeistAugCfg), for the binding's layout check. */
+typedef struct SeistAugCfg {
+  double generate_noise_rate, add_event_rate, shift_event_rate, drop_channel_rate, scale_amplitude_rate;
+  double pre_emphasis_rate, add_noise_rate, add_gap_rate;
+  double coda_ratio, min_snr, p_position_ratio;  /* p_position_ratio in [0, 1]: deterministic cut with P at that ratio */
+  float pre_emphasis_ratio;
+  int32_t in_samples, min_event_gap;             /* min_event_gap in samples */
+  int32_t max_event_num, norm_mode;              /* norm_mode 0 "", 1 "std", 2 "max" */
+  int32_t mask_percent, noise_percent, window;   /* window = sampling_rate // 2 samples, at most 1024 windows per trace */
+} SeistAugCfg;
+uint64_t seist_sizeof_aug(void);
+int seist_aug_recipe_bytes(void);
+int seist_augment(const float* data, int64_t N, int32_t C, int32_t Lin, const int64_t* ppks, const int64_t* spks, int32_t K,
+                  const double* snr, int32_t S, const uint8_t* augment, const SeistAugCfg* cfg, const uint64_t* seed,
+                  float* x, int64_t* ppks_out, int64_t* spks_out, int32_t K_out, uint8_t* cleared, void* work,
+                  int64_t work_bytes, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

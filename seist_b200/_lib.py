@@ -65,6 +65,19 @@ class SeistOp(C.Structure):
     ]
 
 
+class SeistAugCfg(C.Structure):
+    _fields_ = [
+        ("generate_noise_rate", C.c_double), ("add_event_rate", C.c_double), ("shift_event_rate", C.c_double),
+        ("drop_channel_rate", C.c_double), ("scale_amplitude_rate", C.c_double),
+        ("pre_emphasis_rate", C.c_double), ("add_noise_rate", C.c_double), ("add_gap_rate", C.c_double),
+        ("coda_ratio", C.c_double), ("min_snr", C.c_double), ("p_position_ratio", C.c_double),
+        ("pre_emphasis_ratio", C.c_float),
+        ("in_samples", C.c_int32), ("min_event_gap", C.c_int32),
+        ("max_event_num", C.c_int32), ("norm_mode", C.c_int32),
+        ("mask_percent", C.c_int32), ("noise_percent", C.c_int32), ("window", C.c_int32),
+    ]
+
+
 # op kinds (enum SeistOpKind)
 CONV_FWD, CONV_BWD_DATA, CONV_BWD_W, RES_BWD = 1, 2, 3, 4
 ATT_FWD, ATT_BWD_Q, ATT_BWD_KV = 5, 6, 7
@@ -138,6 +151,12 @@ def lib():
     L.seist_dpk_labels.restype = C.c_int
     L.seist_dpk_labels.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_double, C.c_void_p, C.c_void_p]
+    L.seist_sizeof_aug.restype = C.c_uint64
+    L.seist_aug_recipe_bytes.restype = C.c_int
+    L.seist_augment.restype = C.c_int
+    L.seist_augment.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(SeistAugCfg), C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -151,6 +170,8 @@ def lib():
             f"bn {L.seist_sizeof_bn()} vs {C.sizeof(SeistBN)}")
     if L.seist_sizeof_comm() != C.sizeof(SeistComm):
         raise RuntimeError(f"seist_b200: SeistComm layout mismatch {L.seist_sizeof_comm()} vs {C.sizeof(SeistComm)}")
+    if L.seist_sizeof_aug() != C.sizeof(SeistAugCfg):
+        raise RuntimeError(f"seist_b200: SeistAugCfg layout mismatch {L.seist_sizeof_aug()} vs {C.sizeof(SeistAugCfg)}")
     _lib = L
     return L
 
@@ -161,6 +182,7 @@ EXPORTS = [
     "seist_adam_step", "seist_advance_seed", "seist_comm_allreduce", "seist_comm_barrier", "seist_sizeof_comm", "seist_op_family",
     "seist_pick_phase", "seist_detect_event", "seist_pick_counters", "seist_det_counters",
     "seist_normalize", "seist_dpk_labels", "seist_ce_fwd", "seist_ce_bwd",
+    "seist_augment", "seist_sizeof_aug", "seist_aug_recipe_bytes",
 ]
 
 

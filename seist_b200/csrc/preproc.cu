@@ -1,7 +1,8 @@
 // Input side on the device (SURVEY 8f-3): what the reference's DataLoader workers do per waveform in numpy
 // (training/preprocess.py): `_normalize` (:224-242) and the dpk soft labels `_generate_soft_label` (:544-683) with
-// `_pad_phases` (:16-35).  One CTA per trace.  Floating point: double accumulation / double window evaluation, results
-// within 2e-6 of the numpy oracle (oracle/preprocess_ref.py, bit-exactly pinned to the reference's own sources).
+// `_pad_phases` (:16-35), all four window shapes.  One CTA per trace.  Floating point: double accumulation / double
+// window evaluation, results within 2e-6 of the numpy oracle (oracle/preprocess_ref.py, bit-exactly pinned to the
+// reference's own sources; the sigmoid window: tests/augment_ref.py).
 #include "common.cuh"
 
 namespace seist {
@@ -57,6 +58,14 @@ __device__ __forceinline__ double pr_window(int d, int left, int right, int widt
   if (d < -left || d > right) return 0.0;
   if (shape == 0) return exp(-((double)d * (double)d) / 200.0);                     // gaussian, sigma 10 samples
   if (shape == 1) return 1.0 - fabs(2.0 / (double)width * (double)d);               // triangle
+  if (shape == 3) {                                                                 // sigmoid (:586-597)
+    if (d == 0) return 1.0;
+    // left shoulder: 1 / (1 + exp(-10 / left * a)), a = -int(left / 2) + (d + left); right: 10 / right * a, a from
+    // -int(right / 2) at d = 1
+    const double a = d < 0 ? (double)(d + left - left / 2) : (double)(d - 1 - right / 2);
+    const double xv = d < 0 ? __dmul_rn(-10.0 / (double)left, a) : __dmul_rn(-10.0 / (double)right * -1.0, a);
+    return 1.0 / __dadd_rn(1.0, exp(xv));
+  }
   return 1.0;                                                                       // box
 }
 __device__ __forceinline__ double pr_soft(const long long* idx, int n, int j, int L, int left, int right, int width, int shape) {
@@ -135,8 +144,9 @@ int seist_normalize(float* x, int64_t rows, int32_t L, int32_t mode, void* strea
 
 int seist_dpk_labels(const int64_t* ppks, const int64_t* spks, int64_t N, int32_t K, int32_t L, int32_t width, int32_t shape,
                      double coda_ratio, float* out, void* stream) {
-  if (!ppks || !spks || !out || N <= 0 || K < 1 || K > PR_MAXK || L <= 0 || width < 1 || shape < 0 || shape > 2) {
-    set_error("dpk_labels: bad arguments (1 <= K <= 8, shape 0 gaussian / 1 triangle / 2 box)");
+  if (!ppks || !spks || !out || N <= 0 || K < 1 || K > PR_MAXK || L <= 0 || width < 1 || shape < 0 || shape > 3 ||
+      (shape == 3 && width < 2)) {
+    set_error("dpk_labels: bad arguments (1 <= K <= 8, shape 0 gaussian / 1 triangle / 2 box / 3 sigmoid with width >= 2)");
     return -1;
   }
   dpk_labels_kernel<<<(unsigned)N, PR_NT, 0, (cudaStream_t)stream>>>((const long long*)ppks, (const long long*)spks, K, L, width, shape,
