@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 11
+#define SEIST_ABI_VERSION 12
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -292,6 +292,41 @@ int seist_augment(const float* data, int64_t N, int32_t C, int32_t Lin, const in
                   const double* snr, int32_t S, const uint8_t* augment, const SeistAugCfg* cfg, const uint64_t* seed,
                   float* x, int64_t* ppks_out, int64_t* spks_out, int32_t K_out, uint8_t* cleared, void* work,
                   int64_t work_bytes, void* stream);
+
+/* ---- continuous records (DESIGN §4.15): sliding-window inference, overlap stacking, whole-record picking ------------
+   The reference runs one window (demo_predict.py:75 keeps record[:, :8192]); these restate, per window of W samples at
+   stride P, `_normalize` (training/preprocess.py:224-242), and on the stacked traces `_detect_peaks` with topk = None
+   (training/postprocess.py:15-111) and obspy trigger_onset(p, thr, thr) (:114-158) with every run kept.
+   Windows of a station: starts k * P for k = 0 .. (T - W) / P, plus T - W when the last of those ends before T; K per
+   station, window id s * K + k.  record (S, C, T) and probs (S, 3, T) fp32, W <= T < 2^31, 1 <= P <= W.
+   seist_window_batch  = the (B, C, W) model input of windows w0 .. w0 + B - 1, each row normalised as seist_normalize
+                         (mode 0 none, 1 std, 2 max; W <= 49152); ids >= S * K give zero rows.
+   seist_stack_batch   = adds (mode 0) or fmaxf's (mode 1) the (B, 3, W) outputs of windows w0 .. w0 + B - 1 into probs;
+                         each sample takes its covering windows in ascending id order, starting from 0.0f / -inf at its
+                         first covering window.  Call with w0 = 0, B, 2B, ... in order on one stream.
+   seist_stack_finish  = mode 0: probs /= number of covering windows (one IEEE division).
+   seist_peaks_long    = `_detect_peaks(probs[s, channel], mph, mpd > 1, topk=None)` of every row (rising edges, equal
+                         heights: the larger index ranks first); writes counts (S,) int64 and keeps its state in `work`
+                         (seist_peaks_work_bytes).  seist_peaks_long_fill then writes the picks of row s, in index order, at
+                         index / value[offsets[s] ..] (offsets: exclusive prefix sums of counts, int64).
+   seist_runs_long     = the inclusive [on, off] of every maximal run of probs[s, channel] > threshold, in time order:
+                         counts (S,) int64; seist_runs_long_fill writes pairs[offsets[s] ..] (E, 2) int64.
+   The two passes of each pick / run call share `work` and must see the same prob. */
+int seist_window_batch(const float* record, int32_t S, int32_t C, int64_t T, int32_t W, int32_t P, int64_t w0, int32_t B,
+                       int32_t mode, float* x, void* stream);
+int seist_stack_batch(const float* y, int32_t S, int64_t T, int32_t W, int32_t P, int64_t w0, int32_t B, int32_t mode,
+                      float* probs, void* stream);
+int seist_stack_finish(float* probs, int32_t S, int64_t T, int32_t W, int32_t P, void* stream);
+int64_t seist_peaks_work_bytes(int32_t S, int64_t T);
+int seist_peaks_long(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float mph, int32_t min_peak_dist,
+                     void* work, int64_t work_bytes, int64_t* counts, void* stream);
+int seist_peaks_long_fill(int32_t S, int64_t T, const void* work, int64_t work_bytes, const int64_t* offsets, int64_t* index,
+                          float* value, void* stream);
+int64_t seist_runs_work_bytes(int32_t S, int64_t T);
+int seist_runs_long(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float threshold, void* work,
+                    int64_t work_bytes, int64_t* counts, void* stream);
+int seist_runs_long_fill(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float threshold, const void* work,
+                         int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 11
+ABI_VERSION = 12
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -157,6 +157,30 @@ def lib():
     L.seist_augment.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(SeistAugCfg), C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    L.seist_window_batch.restype = C.c_int
+    L.seist_window_batch.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32,
+                                     C.c_int32, C.c_void_p, C.c_void_p]
+    L.seist_stack_batch.restype = C.c_int
+    L.seist_stack_batch.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32,
+                                    C.c_void_p, C.c_void_p]
+    L.seist_stack_finish.restype = C.c_int
+    L.seist_stack_finish.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_void_p]
+    L.seist_peaks_work_bytes.restype = C.c_int64
+    L.seist_peaks_work_bytes.argtypes = [C.c_int32, C.c_int64]
+    L.seist_peaks_long.restype = C.c_int
+    L.seist_peaks_long.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float, C.c_int32, C.c_void_p,
+                                   C.c_int64, C.c_void_p, C.c_void_p]
+    L.seist_peaks_long_fill.restype = C.c_int
+    L.seist_peaks_long_fill.argtypes = [C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]
+    L.seist_runs_work_bytes.restype = C.c_int64
+    L.seist_runs_work_bytes.argtypes = [C.c_int32, C.c_int64]
+    L.seist_runs_long.restype = C.c_int
+    L.seist_runs_long.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_int64,
+                                  C.c_void_p, C.c_void_p]
+    L.seist_runs_long_fill.restype = C.c_int
+    L.seist_runs_long_fill.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float, C.c_void_p,
+                                       C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -183,6 +207,8 @@ EXPORTS = [
     "seist_pick_phase", "seist_detect_event", "seist_pick_counters", "seist_det_counters",
     "seist_normalize", "seist_dpk_labels", "seist_ce_fwd", "seist_ce_bwd",
     "seist_augment", "seist_sizeof_aug", "seist_aug_recipe_bytes",
+    "seist_window_batch", "seist_stack_batch", "seist_stack_finish", "seist_peaks_work_bytes", "seist_peaks_long",
+    "seist_peaks_long_fill", "seist_runs_work_bytes", "seist_runs_long", "seist_runs_long_fill",
 ]
 
 

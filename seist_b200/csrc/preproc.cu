@@ -3,55 +3,17 @@
 // `_pad_phases` (:16-35), all four window shapes.  One CTA per trace.  Floating point: double accumulation / double
 // window evaluation, results within 2e-6 of the numpy oracle (oracle/preprocess_ref.py, bit-exactly pinned to the
 // reference's own sources; the sigmoid window: tests/augment_ref.py).
-#include "common.cuh"
+#include "normalize.cuh"
 
 namespace seist {
 
-constexpr int PR_NT = 256;
 constexpr int PR_MAXK = 8;
 constexpr long long PR_ABSENT = -1000000;     // phase indices below this are "no phase" padding of the (N, K) index tensors
 
-__device__ double pr_block_sum(double v, double* red_s) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red_s[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < PR_NT / 32; ++w) s += red_s[w];
-  return s;
-}
-__device__ float pr_block_max(float v, float* red_s) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red_s[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float s = red_s[0];
-  for (int w = 1; w < PR_NT / 32; ++w) s = fmaxf(s, red_s[w]);
-  return s;
-}
-
-// mode 0: mean removal only, 1: / std (population), 2: / max (signed maximum of the centred trace); zero scale -> 1
+// in place, one CTA per row (pr_normalize_row)
 __global__ void __launch_bounds__(PR_NT) normalize_rows_kernel(float* __restrict__ x, int L, int mode) {
-  __shared__ double red_d[PR_NT / 32];
-  __shared__ float red_f[PR_NT / 32];
   float* row = x + (size_t)blockIdx.x * L;
-  double s = 0.0;
-  for (int i = threadIdx.x; i < L; i += PR_NT) s += (double)row[i];
-  const float mean = (float)(pr_block_sum(s, red_d) / (double)L);
-  float scale = 1.f;
-  if (mode == 1) {
-    double q = 0.0;
-    for (int i = threadIdx.x; i < L; i += PR_NT) { const double d = (double)(row[i] - mean); q += d * d; }
-    scale = (float)sqrt(pr_block_sum(q, red_d) / (double)L);
-  } else if (mode == 2) {
-    float m = -INFINITY;
-    for (int i = threadIdx.x; i < L; i += PR_NT) m = fmaxf(m, row[i] - mean);
-    scale = pr_block_max(m, red_f);
-  }
-  if (scale == 0.f) scale = 1.f;
-  for (int i = threadIdx.x; i < L; i += PR_NT) row[i] = (row[i] - mean) / scale;
+  pr_normalize_row(row, row, L, mode);
 }
 
 __device__ __forceinline__ double pr_window(int d, int left, int right, int width, int shape) {

@@ -1,0 +1,544 @@
+// Continuous records on the device: sliding-window inference input, overlap stacking of the window outputs and
+// whole-record peak picking / event runs (DESIGN §4.15).  The reference has no continuous-data path (demo_predict.py:75
+// keeps the first 8192 samples); per window it is `_normalize` (training/preprocess.py:224-242) -> model -> per trace
+// `_detect_peaks` (training/postprocess.py:15-111, topk = None) and obspy `trigger_onset(p, thr, thr)` (:114-158).
+//
+// Windows of a station of T samples: starts k * P for k = 0 .. Kr - 1, Kr = (T - W) / P + 1, plus one start at T - W
+// when the last of those ends before T; K windows per station, window id s * K + k.
+#include <algorithm>
+
+#include "normalize.cuh"
+
+namespace seist {
+
+constexpr int ST_NT = 256;
+constexpr int ST_CH = ST_NT * 16;      // elements per block of the count / fill passes
+constexpr int ST_SCAN_NT = 1024;
+constexpr int CL_SEG = 1024;           // candidates whose cluster starts a CTA of the cluster pass looks at
+constexpr int CL_SMALL = 32;           // clusters up to this size are resolved by one thread
+constexpr int CL_SMEM = 4096;          // largest cluster staged in shared memory; larger ones stay in global memory
+constexpr unsigned char CL_OPEN = 0, CL_KEEP = 1, CL_DROP = 2;
+
+struct Windows {
+  int T, W, P, Kr, K;
+  __host__ __device__ Windows(int T_, int W_, int P_) : T(T_), W(W_), P(P_) {
+    Kr = (T - W) / P + 1;
+    K = Kr + ((long long)(Kr - 1) * P + W < T ? 1 : 0);
+  }
+  __host__ __device__ int start(int k) const { return k < Kr ? k * P : T - W; }
+  // covering windows of sample t: the regular ones [lo, hi] (empty when lo > hi), then the tail window K - 1 if
+  // t >= T - W and it exists
+  __device__ void cover(int t, int& lo, int& hi, bool& tail) const {
+    lo = t < W ? 0 : (t - W) / P + 1;
+    hi = min(Kr - 1, t / P);
+    tail = K > Kr && t >= T - W;
+  }
+};
+
+// ---- window batch -------------------------------------------------------------------------------------------------
+// x (B, C, W): row (b, c) = normalised record[s, c, start(k):start(k)+W] for window w0 + b = s * K + k; zero past S * K.
+__global__ void __launch_bounds__(PR_NT) window_batch_kernel(const float* __restrict__ rec, int S, int C, Windows win,
+                                                             long long w0, int mode, float* __restrict__ x) {
+  extern __shared__ float wb_row[];                 // [W]: the record slice, read from global memory once
+  const int b = blockIdx.x / C, c = blockIdx.x % C;
+  const long long w = w0 + b;
+  float* dst = x + (size_t)blockIdx.x * win.W;
+  if (w >= (long long)S * win.K) {
+    for (int i = threadIdx.x; i < win.W; i += PR_NT) dst[i] = 0.f;
+    return;
+  }
+  const int s = (int)(w / win.K), k = (int)(w % win.K);
+  const float* src = rec + ((size_t)s * C + c) * win.T + win.start(k);
+  for (int i = threadIdx.x; i < win.W; i += PR_NT) wb_row[i] = src[i];
+  __syncthreads();
+  pr_normalize_row(wb_row, dst, win.W, mode);
+}
+
+// ---- stacking -----------------------------------------------------------------------------------------------------
+// Gather: the thread of probs[s, c, t] adds (maxes) the batch's covering windows of t in ascending window order; the
+// first covering window of t overall starts the accumulator (0.0f + v for the mean, fmaxf(-inf, v) for the max).
+__global__ void __launch_bounds__(ST_NT) stack_batch_kernel(const float* __restrict__ y, int S, Windows win, long long w0,
+                                                            int nb, int s0, int mode, float* __restrict__ probs) {
+  const int s = s0 + blockIdx.y, c = blockIdx.z;
+  const long long wb = (long long)s * win.K;
+  const int ka = (int)max(w0 - wb, 0LL), kb = (int)min(w0 + nb - 1 - wb, (long long)win.K - 1);
+  if (s >= S || ka > kb) return;
+  const int t = win.start(ka) + blockIdx.x * ST_NT + threadIdx.x;
+  if (t >= win.start(kb) + win.W) return;
+  int lo, hi;
+  bool tail;
+  win.cover(t, lo, hi, tail);
+  const int first = lo <= hi ? lo : win.K - 1;
+  float* out = probs + ((size_t)s * 3 + c) * win.T + t;
+  float acc = first >= ka ? (mode == 0 ? 0.f : -INFINITY) : *out;
+  const float* yb = y + (size_t)c * win.W;
+  for (int k = max(lo, ka); k <= min(hi, kb); ++k) {
+    const float v = yb[(size_t)(wb + k - w0) * 3 * win.W + (t - k * win.P)];
+    acc = mode == 0 ? acc + v : fmaxf(acc, v);
+  }
+  if (tail && win.K - 1 >= ka && win.K - 1 <= kb) {
+    const float v = yb[(size_t)(wb + win.K - 1 - w0) * 3 * win.W + (t - (win.T - win.W))];
+    acc = mode == 0 ? acc + v : fmaxf(acc, v);
+  }
+  *out = acc;
+}
+
+// mean: one IEEE division by the number of covering windows
+__global__ void __launch_bounds__(ST_NT) stack_finish_kernel(float* __restrict__ probs, Windows win, long long n) {
+  for (long long i = blockIdx.x * (long long)ST_NT + threadIdx.x; i < n; i += (long long)gridDim.x * ST_NT) {
+    int lo, hi;
+    bool tail;
+    win.cover((int)(i % win.T), lo, hi, tail);
+    const int cnt = max(hi - lo + 1, 0) + (tail ? 1 : 0);
+    probs[i] = __fdiv_rn(probs[i], (float)cnt);
+  }
+}
+
+// ---- order-preserving compaction: per-block counts, a per-row scan of the counts, a fill pass --------------------
+// exclusive rank of this thread's flag among the CTA's flags of one step, and the step's total
+__device__ __forceinline__ int st_block_rank(bool f, int* warp_s, int& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned m = __ballot_sync(0xffffffffu, f);
+  __syncthreads();
+  if (lane == 0) warp_s[warp] = __popc(m);
+  __syncthreads();
+  int base = 0;
+  total = 0;
+  for (int w = 0; w < ST_NT / 32; ++w) {
+    if (w < warp) base += warp_s[w];
+    total += warp_s[w];
+  }
+  return base + __popc(m & ((1u << lane) - 1u));
+}
+
+__device__ __forceinline__ int st_block_count(int v, int* warp_s) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) warp_s[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int s = 0;
+  for (int w = 0; w < ST_NT / 32; ++w) s += warp_s[w];
+  return s;
+}
+
+// blk (rows, nblk): counts -> exclusive offsets in place; total[row]; total64[row] too when given
+__global__ void __launch_bounds__(ST_SCAN_NT) scan_rows_kernel(int* __restrict__ blk, int nblk, int* __restrict__ total,
+                                                               long long* __restrict__ total64) {
+  __shared__ int warp_s[ST_SCAN_NT / 32];
+  __shared__ int carry_s;
+  int* row = blk + (size_t)blockIdx.x * nblk;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) carry_s = 0;
+  __syncthreads();
+  for (int base = 0; base < nblk; base += ST_SCAN_NT) {
+    const int i = base + threadIdx.x;
+    const int v = i < nblk ? row[i] : 0;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += u;
+    }
+    if (lane == 31) warp_s[warp] = inc;
+    __syncthreads();
+    int wbase = 0, tot = 0;
+    for (int w = 0; w < ST_SCAN_NT / 32; ++w) {
+      if (w < warp) wbase += warp_s[w];
+      tot += warp_s[w];
+    }
+    const int carry = carry_s;
+    if (i < nblk) row[i] = carry + wbase + inc - v;
+    __syncthreads();
+    if (threadIdx.x == 0) carry_s = carry + tot;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    total[blockIdx.x] = carry_s;
+    if (total64) total64[blockIdx.x] = carry_s;
+  }
+}
+
+// ---- peaks --------------------------------------------------------------------------------------------------------
+// rising-edge peak candidate (postprocess.py:67-68,82-88): 1 <= i <= T - 2, x[i] - x[i-1] > 0, x[i+1] - x[i] <= 0, x[i] >= mph
+__device__ __forceinline__ bool pk_cand(const float* x, int i, int T, float mph) {
+  if (i < 1 || i > T - 2) return false;
+  const float v = x[i];
+  return v - x[i - 1] > 0.f && x[i + 1] - v <= 0.f && v >= mph;
+}
+
+__global__ void __launch_bounds__(ST_NT) cand_count_kernel(const float* __restrict__ prob, long long n_stride, int T, float mph,
+                                                           int* __restrict__ blk, int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = prob + blockIdx.y * n_stride;
+  const int a = blockIdx.x * ST_CH;
+  int n = 0;
+  for (int i = a + threadIdx.x; i < min(a + ST_CH, T); i += ST_NT) n += pk_cand(x, i, T, mph);
+  n = st_block_count(n, warp_s);
+  if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
+}
+
+__global__ void __launch_bounds__(ST_NT) cand_fill_kernel(const float* __restrict__ prob, long long n_stride, int T, float mph,
+                                                          const int* __restrict__ blk, int nblk, int capc, int* __restrict__ cidx,
+                                                          float* __restrict__ cval) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = prob + blockIdx.y * n_stride;
+  const int a = blockIdx.x * ST_CH;
+  int base = blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  int* ci = cidx + (size_t)blockIdx.y * capc;
+  float* cv = cval + (size_t)blockIdx.y * capc;
+  for (int i0 = a; i0 < min(a + ST_CH, T); i0 += ST_NT) {
+    const int i = i0 + threadIdx.x;
+    const bool f = i < T && pk_cand(x, i, T, mph);
+    int tot;
+    const int r = st_block_rank(f, warp_s, tot);
+    if (f) { ci[base + r] = i; cv[base + r] = x[i]; }
+    base += tot;
+  }
+}
+
+// ranked before: higher value, equal values: larger sample index (oracle/postprocess_ref.py tie rule)
+__device__ __forceinline__ bool pk_above(float vq, int iq, float vk, int ik) { return vq > vk || (vq == vk && iq > ik); }
+
+// Decide candidate k of a cluster if its neighbours within mpd allow it: dropped once a higher-ranked one is kept, kept
+// once every higher-ranked one is dropped.
+__device__ __forceinline__ unsigned char pk_decide(const int* ci, const float* cv, volatile unsigned char* st, int m, int k, int mpd) {
+  const int ik = ci[k];
+  const float vk = cv[k];
+  bool open = false;
+  for (int q = k - 1; q >= 0 && ik - ci[q] <= mpd; --q) {
+    if (!pk_above(cv[q], ci[q], vk, ik)) continue;
+    const unsigned char sq = st[q];
+    if (sq == CL_KEEP) return CL_DROP;
+    open = open || sq == CL_OPEN;
+  }
+  for (int q = k + 1; q < m && ci[q] - ik <= mpd; ++q) {
+    if (!pk_above(cv[q], ci[q], vk, ik)) continue;
+    const unsigned char sq = st[q];
+    if (sq == CL_KEEP) return CL_DROP;
+    open = open || sq == CL_OPEN;
+  }
+  return open ? CL_OPEN : CL_KEEP;
+}
+
+// Greedy suppression of one cluster of m candidates by the whole CTA, as the fixed point of pk_decide.  Decisions are
+// final and only follow from decided neighbours, so a thread may act on neighbours' states of any age: each thread
+// sweeps its contiguous share both ways until it stalls, then the CTA synchronises.  Every round decides at least the
+// highest-ranked open candidate.  ci / cv / st are in shared or global memory.
+__device__ void pk_cluster_cta(const int* ci, const float* cv, volatile unsigned char* st, int m, int mpd) {
+  const int lo = (int)((long long)m * threadIdx.x / ST_NT), hi = (int)((long long)m * (threadIdx.x + 1) / ST_NT);
+  for (;;) {
+    bool changed = true, open = false;
+    while (changed) {
+      changed = false;
+      for (int k = lo; k < hi; ++k)
+        if (st[k] == CL_OPEN) {
+          const unsigned char d = pk_decide(ci, cv, st, m, k, mpd);
+          if (d != CL_OPEN) { st[k] = d; changed = true; }
+        }
+      for (int k = hi - 1; k >= lo; --k)
+        if (st[k] == CL_OPEN) {
+          const unsigned char d = pk_decide(ci, cv, st, m, k, mpd);
+          if (d != CL_OPEN) { st[k] = d; changed = true; }
+        }
+    }
+    for (int k = lo; k < hi; ++k) open = open || st[k] == CL_OPEN;
+    if (!__syncthreads_or(open)) break;
+  }
+}
+
+// Clusters: maximal runs of candidates whose consecutive gaps are <= mpd; a candidate suppresses or is suppressed only
+// inside its cluster.  CTA (seg, row) resolves the clusters that start among candidates [seg * CL_SEG, +CL_SEG): small
+// ones one per thread (greedy in height order), the others together.
+__global__ void __launch_bounds__(ST_NT) cluster_kernel(const int* __restrict__ ncand, int capc, const int* cidx, const float* cval,
+                                                        unsigned char* state, int mpd) {
+  __shared__ int ci_s[CL_SMEM];
+  __shared__ float cv_s[CL_SMEM];
+  __shared__ unsigned char st_s[CL_SMEM];
+  __shared__ int big_s[CL_SEG];
+  __shared__ int nbig_s, end_s;
+  const int n = ncand[blockIdx.y];
+  const int a = blockIdx.x * CL_SEG;
+  if (a >= n) return;
+  const int b = min(a + CL_SEG, n);
+  const int* ci = cidx + (size_t)blockIdx.y * capc;
+  const float* cv = cval + (size_t)blockIdx.y * capc;
+  unsigned char* st = state + (size_t)blockIdx.y * capc;
+  if (threadIdx.x == 0) nbig_s = 0;
+  __syncthreads();
+  for (int j = a + threadIdx.x; j < b; j += ST_NT) {
+    if (j > 0 && ci[j] - ci[j - 1] <= mpd) continue;          // not the first of its cluster
+    int e = j;
+    while (e + 1 < n && ci[e + 1] - ci[e] <= mpd && e - j < CL_SMALL) ++e;
+    if (e - j == CL_SMALL) { big_s[atomicAdd(&nbig_s, 1)] = j; continue; }
+    for (int k = j; k <= e; ++k) st[k] = CL_OPEN;
+    for (;;) {                                                // greedy: keep the best open one, drop its open neighbours
+      int best = -1;
+      for (int k = j; k <= e; ++k)
+        if (st[k] == CL_OPEN && (best < 0 || pk_above(cv[k], ci[k], cv[best], ci[best]))) best = k;
+      if (best < 0) break;
+      st[best] = CL_KEEP;
+      for (int k = j; k <= e; ++k)
+        if (st[k] == CL_OPEN && abs(ci[k] - ci[best]) <= mpd) st[k] = CL_DROP;
+    }
+  }
+  __syncthreads();
+  const int nbig = nbig_s;
+  for (int q = 0; q < nbig; ++q) {
+    const int j = big_s[q];
+    if (threadIdx.x == 0) end_s = n - 1;
+    __syncthreads();
+    for (int base = j; base < n - 1; base += ST_NT) {         // the cluster ends before the first gap > mpd
+      const int k = base + threadIdx.x;
+      if (k < n - 1 && ci[k + 1] - ci[k] > mpd) atomicMin(&end_s, k);
+      if (__syncthreads_or(end_s < n - 1)) break;
+    }
+    const int m = end_s - j + 1;
+    if (m <= CL_SMEM) {
+      for (int k = threadIdx.x; k < m; k += ST_NT) { ci_s[k] = ci[j + k]; cv_s[k] = cv[j + k]; st_s[k] = CL_OPEN; }
+      __syncthreads();
+      pk_cluster_cta(ci_s, cv_s, st_s, m, mpd);
+      for (int k = threadIdx.x; k < m; k += ST_NT) st[j + k] = st_s[k];
+    } else {
+      for (int k = threadIdx.x; k < m; k += ST_NT) st[j + k] = CL_OPEN;
+      __syncthreads();
+      pk_cluster_cta(ci + j, cv + j, st + j, m, mpd);
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(ST_NT) keep_count_kernel(const int* __restrict__ ncand, int capc, const unsigned char* __restrict__ state,
+                                                           int* __restrict__ blk, int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  const int n = ncand[blockIdx.y];
+  const unsigned char* st = state + (size_t)blockIdx.y * capc;
+  const int a = blockIdx.x * ST_CH;
+  int c = 0;
+  for (int j = a + threadIdx.x; j < min(a + ST_CH, n); j += ST_NT) c += st[j] == CL_KEEP;
+  c = st_block_count(c, warp_s);
+  if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = c;
+}
+
+__global__ void __launch_bounds__(ST_NT) keep_fill_kernel(const int* __restrict__ ncand, int capc, const int* __restrict__ cidx,
+                                                          const float* __restrict__ cval, const unsigned char* __restrict__ state,
+                                                          const int* __restrict__ blk, int nblk, const long long* __restrict__ offsets,
+                                                          long long* __restrict__ index, float* __restrict__ value) {
+  __shared__ int warp_s[ST_NT / 32];
+  const int n = ncand[blockIdx.y];
+  const int a = blockIdx.x * ST_CH;
+  if (a >= n) return;
+  const size_t r0 = (size_t)blockIdx.y * capc;
+  long long base = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  for (int j0 = a; j0 < min(a + ST_CH, n); j0 += ST_NT) {
+    const int j = j0 + threadIdx.x;
+    const bool f = j < n && state[r0 + j] == CL_KEEP;
+    int tot;
+    const int r = st_block_rank(f, warp_s, tot);
+    if (f) { index[base + r] = cidx[r0 + j]; value[base + r] = cval[r0 + j]; }
+    base += tot;
+  }
+}
+
+// ---- runs of p > thr ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool rn_on(const float* x, int i, float thr) { return x[i] > thr && (i == 0 || !(x[i - 1] > thr)); }
+__device__ __forceinline__ bool rn_off(const float* x, int i, int T, float thr) { return x[i] > thr && (i == T - 1 || !(x[i + 1] > thr)); }
+
+__global__ void __launch_bounds__(ST_NT) run_count_kernel(const float* __restrict__ prob, long long n_stride, int T, float thr,
+                                                          int* __restrict__ blk, int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = prob + blockIdx.y * n_stride;
+  const int a = blockIdx.x * ST_CH;
+  int n = 0;
+  for (int i = a + threadIdx.x; i < min(a + ST_CH, T); i += ST_NT) n += rn_on(x, i, thr);
+  n = st_block_count(n, warp_s);
+  if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
+}
+
+// blk holds the exclusive run-start offsets per block; the offs before a block are as many, less one when a run crosses
+// into the block
+__global__ void __launch_bounds__(ST_NT) run_fill_kernel(const float* __restrict__ prob, long long n_stride, int T, float thr,
+                                                         const int* __restrict__ blk, int nblk, const long long* __restrict__ offsets,
+                                                         long long* __restrict__ pairs) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = prob + blockIdx.y * n_stride;
+  const int a = blockIdx.x * ST_CH;
+  const long long b0 = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  long long on_base = b0, off_base = b0 - (a > 0 && x[a - 1] > thr && x[a] > thr ? 1 : 0);
+  for (int i0 = a; i0 < min(a + ST_CH, T); i0 += ST_NT) {
+    const int i = i0 + threadIdx.x;
+    const bool fon = i < T && rn_on(x, i, thr), foff = i < T && rn_off(x, i, T, thr);
+    int ton, toff;
+    const int ron = st_block_rank(fon, warp_s, ton);
+    const int roff = st_block_rank(foff, warp_s, toff);
+    if (fon) pairs[(on_base + ron) * 2] = i;
+    if (foff) pairs[(off_base + roff) * 2 + 1] = i;
+    on_base += ton;
+    off_base += toff;
+  }
+}
+
+// ---- work buffers ---------------------------------------------------------------------------------------------------
+__host__ __device__ inline size_t st_align(size_t b) { return (b + 255) & ~(size_t)255; }
+inline int st_capc(int T) { return T / 2 + 1; }                 // candidates of a row: never two adjacent samples
+inline int st_nblk(int n) { return (n + ST_CH - 1) / ST_CH; }
+
+struct PeakWork {
+  int* ncand;
+  int* nkeep;
+  int* blk;
+  int* cidx;
+  float* cval;
+  unsigned char* state;
+  size_t bytes;
+  PeakWork(void* base, int R, int T) {
+    char* p = (char*)base;
+    const size_t capc = st_capc(T);
+    size_t o = 0;
+    ncand = (int*)(p + o);            o += st_align(sizeof(int) * R);
+    nkeep = (int*)(p + o);            o += st_align(sizeof(int) * R);
+    blk = (int*)(p + o);              o += st_align(sizeof(int) * (size_t)R * st_nblk(T));
+    cidx = (int*)(p + o);             o += st_align(sizeof(int) * (size_t)R * capc);
+    cval = (float*)(p + o);           o += st_align(sizeof(float) * (size_t)R * capc);
+    state = (unsigned char*)(p + o);  o += st_align((size_t)R * capc);
+    bytes = o;
+  }
+};
+
+inline size_t run_work_bytes(int R, int T) { return st_align(sizeof(int) * R) + st_align(sizeof(int) * (size_t)R * st_nblk(T)); }
+
+}  // namespace seist
+
+using namespace seist;
+
+extern "C" {
+
+int seist_window_batch(const float* record, int32_t S, int32_t C, int64_t T, int32_t W, int32_t P, int64_t w0, int32_t B,
+                       int32_t mode, float* x, void* stream) {
+  if (!record || !x || S <= 0 || C <= 0 || W < 1 || W > 49152 || T < W || T > INT32_MAX || P < 1 || P > W || w0 < 0 || B <= 0 ||
+      mode < 0 || mode > 2) {
+    set_error("window_batch: bad arguments (W <= T < 2^31, 1 <= W <= 49152, 1 <= P <= W, mode 0 none, 1 std, 2 max)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(window_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  window_batch_kernel<<<(unsigned)((long long)B * C), PR_NT, smem, (cudaStream_t)stream>>>(record, S, C, Windows((int)T, W, P), w0,
+                                                                                           mode, x);
+  note_launch();
+  return check_launch("window_batch");
+}
+
+int seist_stack_batch(const float* y, int32_t S, int64_t T, int32_t W, int32_t P, int64_t w0, int32_t B, int32_t mode, float* probs,
+                      void* stream) {
+  if (!y || !probs || S <= 0 || W < 1 || T < W || T > INT32_MAX || P < 1 || P > W || w0 < 0 || B <= 0 || mode < 0 || mode > 1) {
+    set_error("stack_batch: bad arguments (W <= T < 2^31, 1 <= P <= W, mode 0 mean, 1 max)");
+    return -1;
+  }
+  const Windows win((int)T, W, P);
+  const long long nw = (long long)S * win.K;
+  if (w0 >= nw) return 0;
+  const int nb = (int)std::min<long long>(B, nw - w0);
+  const int s0 = (int)(w0 / win.K), s1 = (int)((w0 + nb - 1) / win.K);
+  const long long span = std::min<long long>(T, (long long)(nb - 1) * P + W);
+  const dim3 grid((unsigned)((span + ST_NT - 1) / ST_NT), (unsigned)(s1 - s0 + 1), 3);
+  stack_batch_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(y, S, win, w0, nb, s0, mode, probs);
+  note_launch();
+  return check_launch("stack_batch");
+}
+
+int seist_stack_finish(float* probs, int32_t S, int64_t T, int32_t W, int32_t P, void* stream) {
+  if (!probs || S <= 0 || W < 1 || T < W || T > INT32_MAX || P < 1 || P > W) {
+    set_error("stack_finish: bad arguments (W <= T < 2^31, 1 <= P <= W)");
+    return -1;
+  }
+  const long long n = (long long)S * 3 * T;
+  const long long g = std::min<long long>((n + ST_NT - 1) / ST_NT, 132LL * 16);
+  stack_finish_kernel<<<(unsigned)g, ST_NT, 0, (cudaStream_t)stream>>>(probs, Windows((int)T, W, P), n);
+  note_launch();
+  return check_launch("stack_finish");
+}
+
+int64_t seist_peaks_work_bytes(int32_t S, int64_t T) {
+  if (S <= 0 || T < 3 || T > INT32_MAX) return -1;
+  return (int64_t)PeakWork(nullptr, S, (int)T).bytes;
+}
+
+int seist_peaks_long(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float mph, int32_t min_peak_dist, void* work,
+                     int64_t work_bytes, int64_t* counts, void* stream) {
+  if (!prob || !work || !counts || S <= 0 || S > 65535 || T < 3 || T > INT32_MAX || channel < 0 || channel >= C || min_peak_dist <= 1 ||
+      work_bytes < seist_peaks_work_bytes(S, T)) {
+    set_error("peaks_long: bad arguments (3 <= T < 2^31, S <= 65535, min_peak_dist > 1, work >= seist_peaks_work_bytes)");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const PeakWork w(work, S, (int)T);
+  const int capc = st_capc((int)T), nblk_t = st_nblk((int)T), nblk_c = st_nblk(capc);
+  const float* x = prob + (size_t)channel * T;
+  const long long ns = (long long)C * T;
+  cand_count_kernel<<<dim3(nblk_t, S), ST_NT, 0, st>>>(x, ns, (int)T, mph, w.blk, nblk_t);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nblk_t, w.ncand, nullptr);
+  cand_fill_kernel<<<dim3(nblk_t, S), ST_NT, 0, st>>>(x, ns, (int)T, mph, w.blk, nblk_t, capc, w.cidx, w.cval);
+  cluster_kernel<<<dim3((capc + CL_SEG - 1) / CL_SEG, S), ST_NT, 0, st>>>(w.ncand, capc, w.cidx, w.cval, w.state, min_peak_dist);
+  keep_count_kernel<<<dim3(nblk_c, S), ST_NT, 0, st>>>(w.ncand, capc, w.state, w.blk, nblk_c);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nblk_c, w.nkeep, (long long*)counts);
+  for (int i = 0; i < 6; ++i) note_launch();
+  return check_launch("peaks_long");
+}
+
+int seist_peaks_long_fill(int32_t S, int64_t T, const void* work, int64_t work_bytes, const int64_t* offsets, int64_t* index, float* value,
+                          void* stream) {
+  if (!work || !offsets || S <= 0 || S > 65535 || T < 3 || T > INT32_MAX || work_bytes < seist_peaks_work_bytes(S, T)) {
+    set_error("peaks_long_fill: bad arguments (the work buffer of the seist_peaks_long call)");
+    return -1;
+  }
+  const PeakWork w(const_cast<void*>(work), S, (int)T);
+  const int capc = st_capc((int)T), nblk_c = st_nblk(capc);
+  keep_fill_kernel<<<dim3(nblk_c, S), ST_NT, 0, (cudaStream_t)stream>>>(w.ncand, capc, w.cidx, w.cval, w.state, w.blk, nblk_c,
+                                                                        (const long long*)offsets, (long long*)index, value);
+  note_launch();
+  return check_launch("peaks_long_fill");
+}
+
+int64_t seist_runs_work_bytes(int32_t S, int64_t T) {
+  if (S <= 0 || T < 1 || T > INT32_MAX) return -1;
+  return (int64_t)run_work_bytes(S, (int)T);
+}
+
+int seist_runs_long(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float threshold, void* work, int64_t work_bytes,
+                    int64_t* counts, void* stream) {
+  if (!prob || !work || !counts || S <= 0 || S > 65535 || T < 1 || T > INT32_MAX || channel < 0 || channel >= C ||
+      work_bytes < seist_runs_work_bytes(S, T)) {
+    set_error("runs_long: bad arguments (1 <= T < 2^31, S <= 65535, work >= seist_runs_work_bytes)");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int* total = (int*)work;
+  int* blk = (int*)((char*)work + st_align(sizeof(int) * S));
+  const int nblk = st_nblk((int)T);
+  run_count_kernel<<<dim3(nblk, S), ST_NT, 0, st>>>(prob + (size_t)channel * T, (long long)C * T, (int)T, threshold, blk, nblk);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(blk, nblk, total, (long long*)counts);
+  note_launch();
+  note_launch();
+  return check_launch("runs_long");
+}
+
+int seist_runs_long_fill(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float threshold, const void* work,
+                         int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream) {
+  if (!prob || !work || !offsets || S <= 0 || S > 65535 || T < 1 || T > INT32_MAX || channel < 0 || channel >= C ||
+      work_bytes < seist_runs_work_bytes(S, T)) {
+    set_error("runs_long_fill: bad arguments (the work buffer of the seist_runs_long call)");
+    return -1;
+  }
+  const int* blk = (const int*)((const char*)work + st_align(sizeof(int) * S));
+  const int nblk = st_nblk((int)T);
+  run_fill_kernel<<<dim3(nblk, S), ST_NT, 0, (cudaStream_t)stream>>>(prob + (size_t)channel * T, (long long)C * T, (int)T, threshold,
+                                                                     blk, nblk, (const long long*)offsets, (long long*)pairs);
+  note_launch();
+  return check_launch("runs_long_fill");
+}
+
+}  // extern "C"

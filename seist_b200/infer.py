@@ -51,5 +51,12 @@ class InferenceGraph:
         if not self.eng.flat.valid():
             raise RuntimeError("the model's parameters were re-allocated (.to()/.cuda()); build a new InferenceGraph")
         self.x.copy_(x, non_blocking=True)
+        return self.replay()
+
+    def replay(self) -> torch.Tensor:
+        """Run the captured plan on the current stream on whatever the static input `self.x` holds (filled in place by
+        the caller's own kernels); returns the static output tensor."""
+        if not self.eng.flat.valid():
+            raise RuntimeError("the model's parameters were re-allocated (.to()/.cuda()); build a new InferenceGraph")
         self.graph.replay()
         return self.y
