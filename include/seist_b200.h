@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 12
+#define SEIST_ABI_VERSION 13
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -327,6 +327,70 @@ int seist_runs_long(const float* prob, int32_t S, int32_t C, int32_t channel, in
                     int64_t work_bytes, int64_t* counts, void* stream);
 int seist_runs_long_fill(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float threshold, const void* work,
                          int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream);
+
+/* ---- continuous records streamed chunk by chunk (DESIGN §4.16) -------------------------------------------------------
+   One call of a stream (a push of n samples per station, or the close) as global int64 sample counts from the start of the
+   stream.  Before the call R = r0 samples were pushed and the samples [0, f0) were emitted; after it R = r1 and [0, f1) are
+   final (f = max(0, R - W) before the close, T at the close).  The call runs the regular windows k0 .. k0 + nk - 1 of every
+   station (start k * P) and, at the close, the tail window starting at `tail` (-1: none); kr is the record's number of
+   regular windows at the close and -1 before.  The call's window j is window j % (nk + (tail >= 0)) of station
+   j / (nk + (tail >= 0)), the tail one last.  Buffers (row-major, fp32):
+     tail_raw  (S, C, W): the last min(W, r0) raw samples, [r0 - min(W, r0), r0); tail_out the same after the call.
+     chunk     (S, C, n = r1 - r0).
+     carry     (S, 3, W): partial sums of [f0, r0); carry_out (S, 3, W) those of [f1, r1) after the call.
+     acc       (S, 3, r1 - f0): the call's partial sums of [f0, r1).
+     probs     (S, 3, f1 - f0): the final probabilities of [f0, f1).
+   seist_stream_window = seist_window_batch for the call's windows j0 .. j0 + B - 1, cut from tail_raw ++ chunk.
+   seist_stream_stack  = seist_stack_batch of those windows' outputs y (B, 3, W) into acc; a sample whose first covering
+                         window ran in an earlier call starts from carry.  Call with j0 = 0, B, 2B, ... in order.
+   seist_stream_emit   = probs (mean: one IEEE division by the number of covering windows; max as is) and carry_out.
+   seist_stream_keep   = tail_out.
+   Picking a stream takes the final probabilities in stretches.  ext (S, C, L) holds, per row, the two samples before the
+   stretch, the stretch and at the close one -inf sentinel; ext sample i is global sample g0 + i.
+   seist_stream_peaks  = the rising-edge candidates of ext[s, channel] at i in [lo, hi] go behind the ones still pending
+                         from the previous call's work `prev` (prev_capc, prev_L; null on the first call), rebased by
+                         -delta; candidates are held as int32 offsets from `base` (candidate i: i + ishift).  Clusters
+                         (gaps <= mpd) whose last candidate c has c + mpd <= lim are resolved as in seist_peaks_long; the
+                         rest stay pending.  counts (S,) int64: picks; info (2S,) int64: pending count, global index of the
+                         first pending candidate (INT64_MAX when none).  work: seist_stream_peaks_work_bytes(S, capc, L);
+                         capc >= max pending + L / 2 + 1.  seist_stream_peaks_fill writes the picks (global index = base +
+                         offset) as seist_peaks_long_fill does.
+   seist_stream_runs   = the runs of ext[s, channel] > threshold that end in this stretch: position p in [lo, hi] closes a
+                         run at p - 1 or opens one at p.  open_in (S,) int64: the start of the run open before the stretch
+                         (-1: none); open_out: the same after it.  counts (S,) int64; work: seist_runs_work_bytes(S, L).
+                         seist_stream_runs_fill writes the [on, off] pairs (global) at pairs[offsets[s] ..]. */
+typedef struct SeistStreamStep {
+  int64_t f0, r0, f1, r1;
+  int64_t k0;          /* first regular window of the call */
+  int64_t tail;        /* start of the tail window run by the call, -1: none */
+  int64_t kr;          /* regular windows of the record (known at the close), -1 before */
+  int32_t S, C, W, P;
+  int32_t nk;          /* regular windows per station run by the call */
+  int32_t norm_mode;   /* 0 none, 1 std, 2 max */
+  int32_t stack_mode;  /* 0 mean, 1 max */
+  int32_t pad_;
+} SeistStreamStep;
+
+uint64_t seist_sizeof_stream_step(void);
+int seist_stream_window(const SeistStreamStep* step, const float* tail_raw, const float* chunk, int64_t j0, int32_t B, float* x,
+                        void* stream);
+int seist_stream_stack(const SeistStreamStep* step, const float* y, int64_t j0, int32_t B, const float* carry, float* acc,
+                       void* stream);
+int seist_stream_emit(const SeistStreamStep* step, const float* carry, const float* acc, float* probs, float* carry_out,
+                      void* stream);
+int seist_stream_keep(const SeistStreamStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream);
+int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L);
+int seist_stream_peaks(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float mph,
+                       int32_t min_peak_dist, int64_t lim, int64_t base, int32_t ishift, void* work, int32_t capc,
+                       const void* prev, int32_t prev_capc, int64_t prev_L, int64_t delta, int32_t max_pend, int64_t* counts,
+                       int64_t* info, void* stream);
+int seist_stream_peaks_fill(int32_t S, int64_t L, const void* work, int32_t capc, int64_t base, const int64_t* offsets,
+                            int64_t* index, float* value, void* stream);
+int seist_stream_runs(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float threshold,
+                      const int64_t* open_in, int64_t* open_out, void* work, int64_t work_bytes, int64_t* counts, void* stream);
+int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi,
+                           float threshold, int64_t g0, const int64_t* open_in, int64_t* open_out, const void* work,
+                           int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

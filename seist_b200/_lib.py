@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 12
+ABI_VERSION = 13
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -75,6 +75,15 @@ class SeistAugCfg(C.Structure):
         ("in_samples", C.c_int32), ("min_event_gap", C.c_int32),
         ("max_event_num", C.c_int32), ("norm_mode", C.c_int32),
         ("mask_percent", C.c_int32), ("noise_percent", C.c_int32), ("window", C.c_int32),
+    ]
+
+
+class SeistStreamStep(C.Structure):
+    _fields_ = [
+        ("f0", C.c_int64), ("r0", C.c_int64), ("f1", C.c_int64), ("r1", C.c_int64),
+        ("k0", C.c_int64), ("tail", C.c_int64), ("kr", C.c_int64),
+        ("S", C.c_int32), ("C", C.c_int32), ("W", C.c_int32), ("P", C.c_int32),
+        ("nk", C.c_int32), ("norm_mode", C.c_int32), ("stack_mode", C.c_int32), ("pad_", C.c_int32),
     ]
 
 
@@ -181,6 +190,32 @@ def lib():
     L.seist_runs_long_fill.restype = C.c_int
     L.seist_runs_long_fill.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float, C.c_void_p,
                                        C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    step = C.POINTER(SeistStreamStep)
+    L.seist_sizeof_stream_step.restype = C.c_uint64
+    L.seist_stream_window.restype = C.c_int
+    L.seist_stream_window.argtypes = [step, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]
+    L.seist_stream_stack.restype = C.c_int
+    L.seist_stream_stack.argtypes = [step, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.seist_stream_emit.restype = C.c_int
+    L.seist_stream_emit.argtypes = [step, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.seist_stream_keep.restype = C.c_int
+    L.seist_stream_keep.argtypes = [step, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.seist_stream_peaks_work_bytes.restype = C.c_int64
+    L.seist_stream_peaks_work_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int64]
+    L.seist_stream_peaks.restype = C.c_int
+    L.seist_stream_peaks.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
+                                     C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                     C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.seist_stream_peaks_fill.restype = C.c_int
+    L.seist_stream_peaks_fill.argtypes = [C.c_int32, C.c_int64, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p]
+    L.seist_stream_runs.restype = C.c_int
+    L.seist_stream_runs.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    L.seist_stream_runs_fill.restype = C.c_int
+    L.seist_stream_runs_fill.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
+                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -196,6 +231,8 @@ def lib():
         raise RuntimeError(f"seist_b200: SeistComm layout mismatch {L.seist_sizeof_comm()} vs {C.sizeof(SeistComm)}")
     if L.seist_sizeof_aug() != C.sizeof(SeistAugCfg):
         raise RuntimeError(f"seist_b200: SeistAugCfg layout mismatch {L.seist_sizeof_aug()} vs {C.sizeof(SeistAugCfg)}")
+    if L.seist_sizeof_stream_step() != C.sizeof(SeistStreamStep):
+        raise RuntimeError(f"seist_b200: SeistStreamStep layout mismatch {L.seist_sizeof_stream_step()} vs {C.sizeof(SeistStreamStep)}")
     _lib = L
     return L
 
@@ -209,6 +246,8 @@ EXPORTS = [
     "seist_augment", "seist_sizeof_aug", "seist_aug_recipe_bytes",
     "seist_window_batch", "seist_stack_batch", "seist_stack_finish", "seist_peaks_work_bytes", "seist_peaks_long",
     "seist_peaks_long_fill", "seist_runs_work_bytes", "seist_runs_long", "seist_runs_long_fill",
+    "seist_sizeof_stream_step", "seist_stream_window", "seist_stream_stack", "seist_stream_emit", "seist_stream_keep",
+    "seist_stream_peaks_work_bytes", "seist_stream_peaks", "seist_stream_peaks_fill", "seist_stream_runs", "seist_stream_runs_fill",
 ]
 
 

@@ -160,39 +160,41 @@ __global__ void __launch_bounds__(ST_SCAN_NT) scan_rows_kernel(int* __restrict__
 }
 
 // ---- peaks --------------------------------------------------------------------------------------------------------
-// rising-edge peak candidate (postprocess.py:67-68,82-88): 1 <= i <= T - 2, x[i] - x[i-1] > 0, x[i+1] - x[i] <= 0, x[i] >= mph
-__device__ __forceinline__ bool pk_cand(const float* x, int i, int T, float mph) {
-  if (i < 1 || i > T - 2) return false;
+// rising-edge peak candidate (postprocess.py:67-68,82-88): x[i] - x[i-1] > 0, x[i+1] - x[i] <= 0, x[i] >= mph; the callers
+// test i in [lo, hi] only (1 .. T - 2 of a whole row; the newly decided samples of a streamed row)
+__device__ __forceinline__ bool pk_cand(const float* x, int i, float mph) {
   const float v = x[i];
   return v - x[i - 1] > 0.f && x[i + 1] - v <= 0.f && v >= mph;
 }
 
-__global__ void __launch_bounds__(ST_NT) cand_count_kernel(const float* __restrict__ prob, long long n_stride, int T, float mph,
+// blocks of ST_CH samples from lo; blk (rows, nblk)
+__global__ void __launch_bounds__(ST_NT) cand_count_kernel(const float* __restrict__ prob, long long n_stride, int lo, int hi, float mph,
                                                            int* __restrict__ blk, int nblk) {
   __shared__ int warp_s[ST_NT / 32];
   const float* x = prob + blockIdx.y * n_stride;
-  const int a = blockIdx.x * ST_CH;
+  const int a = lo + blockIdx.x * ST_CH;
   int n = 0;
-  for (int i = a + threadIdx.x; i < min(a + ST_CH, T); i += ST_NT) n += pk_cand(x, i, T, mph);
+  for (int i = a + threadIdx.x; i < min(a + ST_CH, hi + 1); i += ST_NT) n += pk_cand(x, i, mph);
   n = st_block_count(n, warp_s);
   if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
 }
 
-__global__ void __launch_bounds__(ST_NT) cand_fill_kernel(const float* __restrict__ prob, long long n_stride, int T, float mph,
-                                                          const int* __restrict__ blk, int nblk, int capc, int* __restrict__ cidx,
-                                                          float* __restrict__ cval) {
+// candidate i goes to cidx[row, off0[row] + rank] (off0 may be null: 0) as i + ishift
+__global__ void __launch_bounds__(ST_NT) cand_fill_kernel(const float* __restrict__ prob, long long n_stride, int lo, int hi, float mph,
+                                                          const int* __restrict__ blk, int nblk, const int* __restrict__ off0, int ishift,
+                                                          int capc, int* __restrict__ cidx, float* __restrict__ cval) {
   __shared__ int warp_s[ST_NT / 32];
   const float* x = prob + blockIdx.y * n_stride;
-  const int a = blockIdx.x * ST_CH;
-  int base = blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  const int a = lo + blockIdx.x * ST_CH;
+  int base = blk[(size_t)blockIdx.y * nblk + blockIdx.x] + (off0 ? off0[blockIdx.y] : 0);
   int* ci = cidx + (size_t)blockIdx.y * capc;
   float* cv = cval + (size_t)blockIdx.y * capc;
-  for (int i0 = a; i0 < min(a + ST_CH, T); i0 += ST_NT) {
+  for (int i0 = a; i0 < min(a + ST_CH, hi + 1); i0 += ST_NT) {
     const int i = i0 + threadIdx.x;
-    const bool f = i < T && pk_cand(x, i, T, mph);
+    const bool f = i <= hi && pk_cand(x, i, mph);
     int tot;
     const int r = st_block_rank(f, warp_s, tot);
-    if (f) { ci[base + r] = i; cv[base + r] = x[i]; }
+    if (f) { ci[base + r] = i + ishift; cv[base + r] = x[i]; }
     base += tot;
   }
 }
@@ -323,7 +325,7 @@ __global__ void __launch_bounds__(ST_NT) keep_count_kernel(const int* __restrict
 __global__ void __launch_bounds__(ST_NT) keep_fill_kernel(const int* __restrict__ ncand, int capc, const int* __restrict__ cidx,
                                                           const float* __restrict__ cval, const unsigned char* __restrict__ state,
                                                           const int* __restrict__ blk, int nblk, const long long* __restrict__ offsets,
-                                                          long long* __restrict__ index, float* __restrict__ value) {
+                                                          long long ishift, long long* __restrict__ index, float* __restrict__ value) {
   __shared__ int warp_s[ST_NT / 32];
   const int n = ncand[blockIdx.y];
   const int a = blockIdx.x * ST_CH;
@@ -335,7 +337,7 @@ __global__ void __launch_bounds__(ST_NT) keep_fill_kernel(const int* __restrict_
     const bool f = j < n && state[r0 + j] == CL_KEEP;
     int tot;
     const int r = st_block_rank(f, warp_s, tot);
-    if (f) { index[base + r] = cidx[r0 + j]; value[base + r] = cval[r0 + j]; }
+    if (f) { index[base + r] = cidx[r0 + j] + ishift; value[base + r] = cval[r0 + j]; }
     base += tot;
   }
 }
@@ -378,6 +380,189 @@ __global__ void __launch_bounds__(ST_NT) run_fill_kernel(const float* __restrict
   }
 }
 
+// ---- streamed records (DESIGN §4.16) -------------------------------------------------------------------------------
+// One call of a stream is a SeistStreamStep (include/seist_b200.h); every sample index is a global int64 count.
+__device__ __forceinline__ int ss_nw(const SeistStreamStep& p) { return p.nk + (p.tail >= 0 ? 1 : 0); }
+__device__ __forceinline__ long long ss_start(const SeistStreamStep& p, int q) { return q < p.nk ? (p.k0 + q) * (long long)p.P : p.tail; }
+
+// raw sample g of (s, c): the chunk from r0 on, the kept tail [r0 - min(W, r0), r0) before
+__device__ __forceinline__ float ss_raw(const SeistStreamStep& p, const float* tail, const float* chunk, int s, int c, long long g) {
+  if (g >= p.r0) return chunk[((size_t)s * p.C + c) * (size_t)(p.r1 - p.r0) + (size_t)(g - p.r0)];
+  return tail[((size_t)s * p.C + c) * p.W + (size_t)(g - (p.r0 - min((long long)p.W, (long long)p.r0)))];
+}
+
+// x (B, C, W): row (b, c) = normalised window j0 + b of the call; zero past the call's last window
+__global__ void __launch_bounds__(PR_NT) stream_window_kernel(SeistStreamStep p, const float* __restrict__ tail,
+                                                              const float* __restrict__ chunk, long long j0, float* __restrict__ x) {
+  extern __shared__ float sw_row[];                 // [W]
+  const int b = blockIdx.x / p.C, c = blockIdx.x % p.C;
+  const long long j = j0 + b;
+  const int nw = ss_nw(p);
+  float* dst = x + (size_t)blockIdx.x * p.W;
+  if (j >= (long long)p.S * nw) {
+    for (int i = threadIdx.x; i < p.W; i += PR_NT) dst[i] = 0.f;
+    return;
+  }
+  const int s = (int)(j / nw);
+  const long long a = ss_start(p, (int)(j % nw));
+  for (int i = threadIdx.x; i < p.W; i += PR_NT) sw_row[i] = ss_raw(p, tail, chunk, s, c, a + i);
+  __syncthreads();
+  pr_normalize_row(sw_row, dst, p.W, p.norm_mode);
+}
+
+// tail_out (S, C, W): the last min(W, r1) raw samples after the call
+__global__ void __launch_bounds__(ST_NT) stream_keep_kernel(SeistStreamStep p, const float* __restrict__ tail,
+                                                            const float* __restrict__ chunk, float* __restrict__ tail_out) {
+  const int s = blockIdx.y / p.C, c = blockIdx.y % p.C;
+  const long long keep = min((long long)p.W, (long long)p.r1);
+  const int i = blockIdx.x * ST_NT + threadIdx.x;
+  if (i < keep) tail_out[(size_t)blockIdx.y * p.W + i] = ss_raw(p, tail, chunk, s, c, p.r1 - keep + i);
+}
+
+// stack_batch_kernel for the call's windows j0 .. j0 + nb - 1 into acc ([f0, r1)).  A sample that is not new continues
+// from acc when an earlier batch of the call covered it (the station's part of the batch starts after the call's first
+// window: the window before it covers t), else from carry ([f0, r0), earlier calls)
+__global__ void __launch_bounds__(ST_NT) stream_stack_kernel(SeistStreamStep p, const float* __restrict__ y, long long j0, int nb, int s0,
+                                                             const float* __restrict__ carry, float* __restrict__ acc) {
+  const int s = s0 + blockIdx.y, c = blockIdx.z;
+  const int nw = ss_nw(p);
+  const long long wb = (long long)s * nw;
+  const int qa = (int)max(j0 - wb, 0LL), qb = (int)min(j0 + nb - 1 - wb, (long long)nw - 1);
+  if (s >= p.S || qa > qb) return;
+  const long long t = ss_start(p, qa) + blockIdx.x * (long long)ST_NT + threadIdx.x;
+  if (t >= ss_start(p, qb) + p.W) return;
+  const long long lo = t < p.W ? 0 : (t - p.W) / p.P + 1, hi = min(t / p.P, (long long)p.k0 + p.nk - 1);
+  const bool reg = lo <= hi;                                   // else the tail window is t's only one
+  const bool tl = p.tail >= 0 && qb == nw - 1 && t >= p.tail;
+  const long long kqa = p.k0 + qa;
+  const bool first = reg ? (qa < p.nk && lo >= kqa) : tl;
+  float* out = acc + ((size_t)s * 3 + c) * (size_t)(p.r1 - p.f0) + (size_t)(t - p.f0);
+  float a = first ? (p.stack_mode == 0 ? 0.f : -INFINITY)
+                  : (qa > 0 ? *out : carry[((size_t)s * 3 + c) * p.W + (size_t)(t - p.f0)]);   // window k0 + qa - 1 covers t
+  const float* yb = y + (size_t)c * p.W;
+  const long long kb = min(hi, (long long)p.k0 + min(qb, p.nk - 1));
+  for (long long k = max(lo, kqa); k <= kb; ++k) {
+    const float v = yb[(size_t)(wb + (k - p.k0) - j0) * 3 * p.W + (size_t)(t - k * p.P)];
+    a = p.stack_mode == 0 ? a + v : fmaxf(a, v);
+  }
+  if (tl) {
+    const float v = yb[(size_t)(wb + p.nk - j0) * 3 * p.W + (size_t)(t - p.tail)];
+    a = p.stack_mode == 0 ? a + v : fmaxf(a, v);
+  }
+  *out = a;
+}
+
+// probs = final [f0, f1) (the mean divided once by its number of covering windows), carry_out = partial sums of [f1, r1)
+__global__ void __launch_bounds__(ST_NT) stream_emit_kernel(SeistStreamStep p, const float* __restrict__ carry, const float* __restrict__ acc,
+                                                            float* __restrict__ probs, float* __restrict__ carry_out) {
+  const long long L = p.r1 - p.f0, n = (long long)p.S * 3 * L;
+  const long long run_lo = p.k0 * p.P, run_hi = (p.k0 + p.nk - 1) * p.P + p.W;
+  for (long long i = blockIdx.x * (long long)ST_NT + threadIdx.x; i < n; i += (long long)gridDim.x * ST_NT) {
+    const long long row = i / L, t = p.f0 + i % L;
+    const bool touched = (p.nk > 0 && t >= run_lo && t < run_hi) || (p.tail >= 0 && t >= p.tail);
+    float v = touched ? acc[i] : (t < p.r0 ? carry[row * p.W + (t - p.f0)] : 0.f);   // t >= r0 untouched: no window yet
+    if (t < p.f1) {
+      if (p.stack_mode == 0) {
+        const long long lo = t < p.W ? 0 : (t - p.W) / p.P + 1, hi = p.kr >= 0 ? min(t / p.P, (long long)p.kr - 1) : t / p.P;
+        const int cnt = (int)max(hi - lo + 1, 0LL) + (p.tail >= 0 && t >= p.tail ? 1 : 0);
+        v = __fdiv_rn(v, (float)cnt);
+      }
+      probs[row * (p.f1 - p.f0) + (t - p.f0)] = v;
+    } else {
+      carry_out[row * p.W + (t - p.f1)] = v;
+    }
+  }
+}
+
+// pending candidates of the previous call ([nclosed, ncand) of its rows) to the front of this call's rows, rebased
+__global__ void __launch_bounds__(ST_NT) pend_move_kernel(const int* __restrict__ pci, const float* __restrict__ pcv, int pcapc,
+                                                          const int* __restrict__ pnclosed, const int* __restrict__ pncand, long long delta,
+                                                          int* __restrict__ cidx, float* __restrict__ cval, int capc, int* __restrict__ npend) {
+  const int s = blockIdx.y;
+  const int a = pci ? pnclosed[s] : 0, m = pci ? pncand[s] - a : 0;
+  if (blockIdx.x == 0 && threadIdx.x == 0) npend[s] = m;
+  for (int j = blockIdx.x * ST_NT + threadIdx.x; j < m; j += gridDim.x * ST_NT) {
+    cidx[(size_t)s * capc + j] = (int)(pci[(size_t)s * pcapc + a + j] - delta);
+    cval[(size_t)s * capc + j] = pcv[(size_t)s * pcapc + a + j];
+  }
+}
+
+// per row: ncand = pending + new; the closed prefix ends before the last cluster unless its last candidate c has
+// c + mpd <= lim (no later candidate can join it); info = (pending count, global index of the first pending one)
+__global__ void __launch_bounds__(ST_NT) close_scan_kernel(const int* __restrict__ npend, const int* __restrict__ nnew, const int* __restrict__ cidx,
+                                                           int capc, int mpd, long long lim, long long base, int* __restrict__ ncand,
+                                                           int* __restrict__ nclosed, long long* __restrict__ info) {
+  __shared__ int last_s;
+  const int s = blockIdx.x, n = npend[s] + nnew[s];
+  const int* ci = cidx + (size_t)s * capc;
+  if (threadIdx.x == 0) last_s = 0;
+  __syncthreads();
+  for (int top = n - 1; top >= 1; top -= ST_NT) {            // the last cluster start, searched from the end
+    const int j = top - (int)threadIdx.x;
+    const bool f = j >= 1 && ci[j] - ci[j - 1] > mpd;
+    if (f) atomicMax(&last_s, j);
+    if (__syncthreads_or(f)) break;
+  }
+  if (threadIdx.x == 0) {
+    const int nc = n == 0 || (long long)ci[n - 1] + mpd <= lim ? n : last_s;
+    ncand[s] = n;
+    nclosed[s] = nc;
+    info[s] = n - nc;
+    info[gridDim.x + s] = nc < n ? base + ci[nc] : LLONG_MAX;
+  }
+}
+
+// runs of a streamed row: position p closes a run at p - 1 (sr_off) or opens one at p (sr_on); x[lo - 1] is the last
+// sample of the previous stretch
+__device__ __forceinline__ bool sr_off(const float* x, int p, float thr) { return x[p - 1] > thr && !(x[p] > thr); }
+__device__ __forceinline__ bool sr_on(const float* x, int p, float thr) { return x[p] > thr && !(x[p - 1] > thr); }
+
+__global__ void __launch_bounds__(ST_NT) srun_count_kernel(const float* __restrict__ prob, long long n_stride, int lo, int hi, float thr,
+                                                           int* __restrict__ blk, int nblk, const long long* __restrict__ open_in,
+                                                           long long* __restrict__ open_out) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = prob + blockIdx.y * n_stride;
+  const int a = lo + blockIdx.x * ST_CH;
+  int n = 0;
+  for (int i = a + threadIdx.x; i < min(a + ST_CH, hi + 1); i += ST_NT) n += sr_off(x, i, thr);
+  n = st_block_count(n, warp_s);
+  if (threadIdx.x == 0) {
+    blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
+    if (blockIdx.x == 0) open_out[blockIdx.y] = x[hi] > thr ? open_in[blockIdx.y] : -1;   // raised by srun_fill on a new start
+  }
+}
+
+// blk: exclusive counts of run ends before each block.  The run ending at the k-th end of the row is pair offsets[s] + k;
+// the carried open run is the first of them.
+__global__ void __launch_bounds__(ST_NT) srun_fill_kernel(const float* __restrict__ prob, long long n_stride, int lo, int hi, float thr,
+                                                          long long g0, const int* __restrict__ blk, int nblk,
+                                                          const long long* __restrict__ offsets, const long long* __restrict__ open_in,
+                                                          long long* __restrict__ open_out, long long* __restrict__ pairs) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = prob + blockIdx.y * n_stride;
+  const int a = lo + blockIdx.x * ST_CH;
+  const long long end = offsets[blockIdx.y + 1];
+  if (blockIdx.x == 0 && threadIdx.x == 0 && open_in[blockIdx.y] >= 0 && end > offsets[blockIdx.y])
+    pairs[offsets[blockIdx.y] * 2] = open_in[blockIdx.y];
+  const bool open_end = x[hi] > thr;
+  long long off_base = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  long long on_base = off_base + (x[a - 1] > thr ? 1 : 0);    // a run open into the block ends before the next starts
+  for (int i0 = a; i0 < min(a + ST_CH, hi + 1); i0 += ST_NT) {
+    const int i = i0 + threadIdx.x;
+    const bool fon = i <= hi && sr_on(x, i, thr), foff = i <= hi && sr_off(x, i, thr);
+    int ton, toff;
+    const int ron = st_block_rank(fon, warp_s, ton);
+    const int roff = st_block_rank(foff, warp_s, toff);
+    if (foff) pairs[(off_base + roff) * 2 + 1] = g0 + i - 1;
+    if (fon) {
+      if (on_base + ron < end) pairs[(on_base + ron) * 2] = g0 + i;
+      else if (open_end) atomicMax(&open_out[blockIdx.y], g0 + i);
+    }
+    on_base += ton;
+    off_base += toff;
+  }
+}
+
 // ---- work buffers ---------------------------------------------------------------------------------------------------
 __host__ __device__ inline size_t st_align(size_t b) { return (b + 255) & ~(size_t)255; }
 inline int st_capc(int T) { return T / 2 + 1; }                 // candidates of a row: never two adjacent samples
@@ -398,6 +583,35 @@ struct PeakWork {
     ncand = (int*)(p + o);            o += st_align(sizeof(int) * R);
     nkeep = (int*)(p + o);            o += st_align(sizeof(int) * R);
     blk = (int*)(p + o);              o += st_align(sizeof(int) * (size_t)R * st_nblk(T));
+    cidx = (int*)(p + o);             o += st_align(sizeof(int) * (size_t)R * capc);
+    cval = (float*)(p + o);           o += st_align(sizeof(float) * (size_t)R * capc);
+    state = (unsigned char*)(p + o);  o += st_align((size_t)R * capc);
+    bytes = o;
+  }
+};
+
+struct StreamPeakWork {
+  int* npend;
+  int* nnew;
+  int* ncand;
+  int* nclosed;
+  int* nkeep;
+  int* blk;
+  int* cidx;
+  float* cval;
+  unsigned char* state;
+  int nblk;
+  size_t bytes;
+  StreamPeakWork(const void* base, int R, int capc, long long L) {
+    char* p = (char*)base;
+    nblk = std::max(st_nblk((int)L), st_nblk(capc));
+    size_t o = 0;
+    npend = (int*)(p + o);            o += st_align(sizeof(int) * R);
+    nnew = (int*)(p + o);             o += st_align(sizeof(int) * R);
+    ncand = (int*)(p + o);            o += st_align(sizeof(int) * R);
+    nclosed = (int*)(p + o);          o += st_align(sizeof(int) * R);
+    nkeep = (int*)(p + o);            o += st_align(sizeof(int) * R);
+    blk = (int*)(p + o);              o += st_align(sizeof(int) * (size_t)R * nblk);
     cidx = (int*)(p + o);             o += st_align(sizeof(int) * (size_t)R * capc);
     cval = (float*)(p + o);           o += st_align(sizeof(float) * (size_t)R * capc);
     state = (unsigned char*)(p + o);  o += st_align((size_t)R * capc);
@@ -479,9 +693,9 @@ int seist_peaks_long(const float* prob, int32_t S, int32_t C, int32_t channel, i
   const int capc = st_capc((int)T), nblk_t = st_nblk((int)T), nblk_c = st_nblk(capc);
   const float* x = prob + (size_t)channel * T;
   const long long ns = (long long)C * T;
-  cand_count_kernel<<<dim3(nblk_t, S), ST_NT, 0, st>>>(x, ns, (int)T, mph, w.blk, nblk_t);
+  cand_count_kernel<<<dim3(nblk_t, S), ST_NT, 0, st>>>(x, ns, 1, (int)T - 2, mph, w.blk, nblk_t);
   scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nblk_t, w.ncand, nullptr);
-  cand_fill_kernel<<<dim3(nblk_t, S), ST_NT, 0, st>>>(x, ns, (int)T, mph, w.blk, nblk_t, capc, w.cidx, w.cval);
+  cand_fill_kernel<<<dim3(nblk_t, S), ST_NT, 0, st>>>(x, ns, 1, (int)T - 2, mph, w.blk, nblk_t, nullptr, 0, capc, w.cidx, w.cval);
   cluster_kernel<<<dim3((capc + CL_SEG - 1) / CL_SEG, S), ST_NT, 0, st>>>(w.ncand, capc, w.cidx, w.cval, w.state, min_peak_dist);
   keep_count_kernel<<<dim3(nblk_c, S), ST_NT, 0, st>>>(w.ncand, capc, w.state, w.blk, nblk_c);
   scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nblk_c, w.nkeep, (long long*)counts);
@@ -498,7 +712,7 @@ int seist_peaks_long_fill(int32_t S, int64_t T, const void* work, int64_t work_b
   const PeakWork w(const_cast<void*>(work), S, (int)T);
   const int capc = st_capc((int)T), nblk_c = st_nblk(capc);
   keep_fill_kernel<<<dim3(nblk_c, S), ST_NT, 0, (cudaStream_t)stream>>>(w.ncand, capc, w.cidx, w.cval, w.state, w.blk, nblk_c,
-                                                                        (const long long*)offsets, (long long*)index, value);
+                                                                        (const long long*)offsets, 0, (long long*)index, value);
   note_launch();
   return check_launch("peaks_long_fill");
 }
@@ -539,6 +753,162 @@ int seist_runs_long_fill(const float* prob, int32_t S, int32_t C, int32_t channe
                                                                      blk, nblk, (const long long*)offsets, (long long*)pairs);
   note_launch();
   return check_launch("runs_long_fill");
+}
+
+uint64_t seist_sizeof_stream_step(void) { return sizeof(SeistStreamStep); }
+
+static bool ss_ok(const SeistStreamStep* p) {
+  return p && p->S > 0 && p->S <= 65535 && p->C > 0 && p->W >= 1 && p->W <= 49152 && p->P >= 1 && p->P <= p->W && p->f0 >= 0 &&
+         p->r0 >= p->f0 && p->r0 - p->f0 <= p->W && p->r1 >= p->r0 && p->f1 >= p->f0 && p->f1 <= p->r1 && p->r1 - p->f1 <= p->W &&
+         p->r1 - p->f0 <= INT32_MAX && p->k0 >= 0 && p->nk >= 0 && p->norm_mode >= 0 && p->norm_mode <= 2 && p->stack_mode >= 0 &&
+         p->stack_mode <= 1 && (p->nk == 0 || (p->k0 + p->nk - 1) * p->P + p->W <= p->r1) &&
+         (p->tail < 0 || (p->tail >= p->r1 - p->W && p->tail + p->W == p->r1 && p->kr >= 0));
+}
+
+int seist_stream_window(const SeistStreamStep* step, const float* tail_raw, const float* chunk, int64_t j0, int32_t B, float* x,
+                        void* stream) {
+  if (!ss_ok(step) || !x || j0 < 0 || B <= 0 || (step->r0 > 0 && !tail_raw) || (step->r1 > step->r0 && !chunk)) {
+    set_error("stream_window: bad arguments (a consistent SeistStreamStep, W <= 49152, j0 >= 0, B > 0)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * step->W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(stream_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  stream_window_kernel<<<(unsigned)((long long)B * step->C), PR_NT, smem, (cudaStream_t)stream>>>(*step, tail_raw, chunk, j0, x);
+  note_launch();
+  return check_launch("stream_window");
+}
+
+int seist_stream_stack(const SeistStreamStep* step, const float* y, int64_t j0, int32_t B, const float* carry, float* acc,
+                       void* stream) {
+  if (!ss_ok(step) || !y || !carry || !acc || j0 < 0 || B <= 0) {
+    set_error("stream_stack: bad arguments (a consistent SeistStreamStep, j0 >= 0, B > 0)");
+    return -1;
+  }
+  const SeistStreamStep& p = *step;
+  const long long nw = p.nk + (p.tail >= 0 ? 1 : 0), total = (long long)p.S * nw;
+  if (j0 >= total) return 0;
+  const int nb = (int)std::min<long long>(B, total - j0);
+  const int s0 = (int)(j0 / nw), s1 = (int)((j0 + nb - 1) / nw);
+  const long long span = std::min<long long>(p.r1 - p.f0, (long long)(nb - 1) * p.P + p.W);
+  const dim3 grid((unsigned)((span + ST_NT - 1) / ST_NT), (unsigned)(s1 - s0 + 1), 3);
+  stream_stack_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(p, y, j0, nb, s0, carry, acc);
+  note_launch();
+  return check_launch("stream_stack");
+}
+
+int seist_stream_emit(const SeistStreamStep* step, const float* carry, const float* acc, float* probs, float* carry_out,
+                      void* stream) {
+  if (!ss_ok(step) || !carry || !carry_out || (step->r1 > step->f0 && !acc) || (step->f1 > step->f0 && !probs)) {
+    set_error("stream_emit: bad arguments (a consistent SeistStreamStep)");
+    return -1;
+  }
+  const long long n = (long long)step->S * 3 * (step->r1 - step->f0);
+  if (n == 0) return 0;
+  const long long g = std::min<long long>((n + ST_NT - 1) / ST_NT, 132LL * 16);
+  stream_emit_kernel<<<(unsigned)g, ST_NT, 0, (cudaStream_t)stream>>>(*step, carry, acc, probs, carry_out);
+  note_launch();
+  return check_launch("stream_emit");
+}
+
+int seist_stream_keep(const SeistStreamStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream) {
+  if (!ss_ok(step) || !tail_out || (step->r0 > 0 && !tail_raw) || (step->r1 > step->r0 && !chunk) || step->S * step->C > 65535) {
+    set_error("stream_keep: bad arguments (a consistent SeistStreamStep, S * C <= 65535)");
+    return -1;
+  }
+  const long long keep = std::min<long long>(step->W, step->r1);
+  if (keep == 0) return 0;
+  stream_keep_kernel<<<dim3((unsigned)((keep + ST_NT - 1) / ST_NT), step->S * step->C), ST_NT, 0, (cudaStream_t)stream>>>(
+      *step, tail_raw, chunk, tail_out);
+  note_launch();
+  return check_launch("stream_keep");
+}
+
+int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L) {
+  if (S <= 0 || capc < 1 || L < 2 || L > INT32_MAX) return -1;
+  return (int64_t)StreamPeakWork(nullptr, S, capc, L).bytes;
+}
+
+int seist_stream_peaks(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float mph,
+                       int32_t min_peak_dist, int64_t lim, int64_t base, int32_t ishift, void* work, int32_t capc,
+                       const void* prev, int32_t prev_capc, int64_t prev_L, int64_t delta, int32_t max_pend, int64_t* counts,
+                       int64_t* info, void* stream) {
+  if (!ext || !work || !counts || !info || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || channel < 0 || channel >= C ||
+      lo < 1 || hi > L - 2 || min_peak_dist <= 1 || ishift < 0 || max_pend < 0 || capc < max_pend + (int)(L / 2) + 1 ||
+      (prev && (prev_capc < 1 || prev_L < 2 || prev_L > INT32_MAX))) {
+    set_error("stream_peaks: bad arguments (1 <= lo, hi <= L - 2, S <= 65535, min_peak_dist > 1, capc >= max_pend + L / 2 + 1)");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const StreamPeakWork w(work, S, capc, L);
+  const float* x = ext + (size_t)channel * L;
+  const long long ns = (long long)C * L;
+  const int nb = std::max(1, st_nblk(hi - lo + 1)), nbc = st_nblk(capc);
+  const StreamPeakWork pw(prev, S, prev ? prev_capc : 1, prev ? prev_L : 2);
+  pend_move_kernel<<<dim3(std::max(1, (max_pend + ST_NT - 1) / ST_NT), S), ST_NT, 0, st>>>(
+      prev ? pw.cidx : nullptr, pw.cval, prev_capc, pw.nclosed, pw.ncand, delta, w.cidx, w.cval, capc, w.npend);
+  cand_count_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(x, ns, lo, hi, mph, w.blk, nb);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nb, w.nnew, nullptr);
+  cand_fill_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(x, ns, lo, hi, mph, w.blk, nb, w.npend, ishift, capc, w.cidx, w.cval);
+  close_scan_kernel<<<S, ST_NT, 0, st>>>(w.npend, w.nnew, w.cidx, capc, min_peak_dist, lim, base, w.ncand, w.nclosed, (long long*)info);
+  cluster_kernel<<<dim3((capc + CL_SEG - 1) / CL_SEG, S), ST_NT, 0, st>>>(w.nclosed, capc, w.cidx, w.cval, w.state, min_peak_dist);
+  keep_count_kernel<<<dim3(nbc, S), ST_NT, 0, st>>>(w.nclosed, capc, w.state, w.blk, nbc);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nbc, w.nkeep, (long long*)counts);
+  for (int i = 0; i < 8; ++i) note_launch();
+  return check_launch("stream_peaks");
+}
+
+int seist_stream_peaks_fill(int32_t S, int64_t L, const void* work, int32_t capc, int64_t base, const int64_t* offsets,
+                            int64_t* index, float* value, void* stream) {
+  if (!work || !offsets || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || capc < 1) {
+    set_error("stream_peaks_fill: bad arguments (the work buffer of the seist_stream_peaks call)");
+    return -1;
+  }
+  const StreamPeakWork w(work, S, capc, L);
+  const int nbc = st_nblk(capc);
+  keep_fill_kernel<<<dim3(nbc, S), ST_NT, 0, (cudaStream_t)stream>>>(w.nclosed, capc, w.cidx, w.cval, w.state, w.blk, nbc,
+                                                                     (const long long*)offsets, base, (long long*)index, value);
+  note_launch();
+  return check_launch("stream_peaks_fill");
+}
+
+int seist_stream_runs(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float threshold,
+                      const int64_t* open_in, int64_t* open_out, void* work, int64_t work_bytes, int64_t* counts, void* stream) {
+  if (!ext || !work || !counts || !open_in || !open_out || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || channel < 0 ||
+      channel >= C || lo < 1 || hi > L - 1 || hi < lo - 1 || work_bytes < seist_runs_work_bytes(S, L)) {
+    set_error("stream_runs: bad arguments (1 <= lo, lo - 1 <= hi <= L - 1, S <= 65535, work >= seist_runs_work_bytes)");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int* total = (int*)work;
+  int* blk = (int*)((char*)work + st_align(sizeof(int) * S));
+  const int nb = std::max(1, st_nblk(hi - lo + 1));
+  srun_count_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(ext + (size_t)channel * L, (long long)C * L, lo, hi, threshold, blk, nb,
+                                                  (const long long*)open_in, (long long*)open_out);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(blk, nb, total, (long long*)counts);
+  note_launch();
+  note_launch();
+  return check_launch("stream_runs");
+}
+
+int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi,
+                           float threshold, int64_t g0, const int64_t* open_in, int64_t* open_out, const void* work,
+                           int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream) {
+  if (!ext || !work || !offsets || !open_in || !open_out || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || channel < 0 ||
+      channel >= C || lo < 1 || hi > L - 1 || hi < lo - 1 || work_bytes < seist_runs_work_bytes(S, L)) {
+    set_error("stream_runs_fill: bad arguments (the work buffer of the seist_stream_runs call)");
+    return -1;
+  }
+  const int* blk = (const int*)((const char*)work + st_align(sizeof(int) * S));
+  const int nb = std::max(1, st_nblk(hi - lo + 1));
+  srun_fill_kernel<<<dim3(nb, S), ST_NT, 0, (cudaStream_t)stream>>>(ext + (size_t)channel * L, (long long)C * L, lo, hi, threshold, g0,
+                                                                    blk, nb, (const long long*)offsets, (const long long*)open_in,
+                                                                    (long long*)open_out, (long long*)pairs);
+  note_launch();
+  return check_launch("stream_runs_fill");
 }
 
 }  // extern "C"

@@ -13,7 +13,7 @@ the covering windows).  Picks are `_detect_peaks(mph=threshold, mpd=min_peak_dis
 """
 from __future__ import annotations
 
-from typing import List, Tuple
+from typing import List, NamedTuple, Tuple
 
 import torch
 
@@ -142,6 +142,262 @@ def detect_runs(probs: torch.Tensor, channel: int, threshold: float):
     return pairs, off
 
 
+# ---- streamed records (DESIGN §4.16) ---------------------------------------------------------------------------------
+_I64_MAX = (1 << 63) - 1
+_I32_MAX = (1 << 31) - 1
+
+
+def stream_step(S: int, C: int, window: int, stride: int, f0: int, r0: int, f1: int, r1: int, k0: int, nk: int, tail: int = -1,
+                kr: int = -1, norm_mode: str = "std", stack: str = "mean") -> _lib.SeistStreamStep:
+    """One call of a stream as global sample counts (include/seist_b200.h, SeistStreamStep): R goes r0 -> r1, the final
+    prefix f0 -> f1; the call runs regular windows k0 .. k0 + nk - 1 of every station and, at the close, the tail window
+    starting at `tail` (-1: none) of a record with kr regular windows."""
+    return _lib.SeistStreamStep(f0=f0, r0=r0, f1=f1, r1=r1, k0=k0, tail=tail, kr=kr, S=S, C=C, W=window, P=stride, nk=nk,
+                                norm_mode=_MODES[norm_mode], stack_mode=_STACK[stack])
+
+
+def _ref(step):
+    import ctypes
+    return ctypes.byref(step)
+
+
+def stream_window_(x: torch.Tensor, step, tail_raw: torch.Tensor, chunk: torch.Tensor | None, j0: int) -> torch.Tensor:
+    """Fill x (B, C, W) with the normalised windows j0 .. j0 + B - 1 of the call `step`, cut from tail_raw (S, C, W) (the
+    last min(W, r0) raw samples) followed by chunk (S, C, r1 - r0); ids past the call's last window give zero rows."""
+    S, C, W = step.S, step.C, step.W
+    _dense(tail_raw, (S, C, W), "kept raw samples")
+    _dense(x, (None, C, W), "window batch", tail_raw.device)
+    if step.r1 > step.r0:
+        _dense(chunk, (S, C, step.r1 - step.r0), "chunk", tail_raw.device)
+    _lib.check(_lib.lib().seist_stream_window(_ref(step), tail_raw.data_ptr(), chunk.data_ptr() if step.r1 > step.r0 else None, j0,
+                                              x.shape[0], x.data_ptr(), _s()), "seist_stream_window")
+    return x
+
+
+def stream_stack_(acc: torch.Tensor, y: torch.Tensor, step, j0: int, carry: torch.Tensor) -> torch.Tensor:
+    """Stack the (B, 3, W) outputs of the call's windows j0 .. j0 + B - 1 into acc (S, 3, r1 - f0); carry (S, 3, W) holds the
+    partial sums of [f0, r0) from earlier calls.  Batches in order from j0 = 0."""
+    S, W = step.S, step.W
+    _dense(carry, (S, 3, W), "carry")
+    _dense(acc, (S, 3, step.r1 - step.f0), "partial sums", carry.device)
+    _dense(y, (None, 3, W), "window outputs", carry.device)
+    _lib.check(_lib.lib().seist_stream_stack(_ref(step), y.data_ptr(), j0, y.shape[0], carry.data_ptr(), acc.data_ptr(), _s()),
+               "seist_stream_stack")
+    return acc
+
+
+def stream_emit_(probs: torch.Tensor, carry_out: torch.Tensor, step, carry: torch.Tensor, acc: torch.Tensor) -> torch.Tensor:
+    """probs (S, 3, f1 - f0) = the final probabilities of [f0, f1); carry_out (S, 3, W) = the partial sums of [f1, r1)."""
+    S, W = step.S, step.W
+    _dense(carry, (S, 3, W), "carry")
+    _dense(carry_out, (S, 3, W), "carry_out", carry.device)
+    _dense(acc, (S, 3, step.r1 - step.f0), "partial sums", carry.device)
+    _dense(probs, (S, 3, step.f1 - step.f0), "probs", carry.device)
+    if carry_out.data_ptr() == carry.data_ptr():
+        raise ValueError("carry_out must not be carry")
+    _lib.check(_lib.lib().seist_stream_emit(_ref(step), carry.data_ptr(), acc.data_ptr(), probs.data_ptr(), carry_out.data_ptr(), _s()),
+               "seist_stream_emit")
+    return probs
+
+
+def stream_keep_(tail_out: torch.Tensor, step, tail_raw: torch.Tensor, chunk: torch.Tensor | None) -> torch.Tensor:
+    """tail_out (S, C, W) = the last min(W, r1) raw samples after the call."""
+    S, C, W = step.S, step.C, step.W
+    _dense(tail_raw, (S, C, W), "kept raw samples")
+    _dense(tail_out, (S, C, W), "tail_out", tail_raw.device)
+    if step.r1 > step.r0:
+        _dense(chunk, (S, C, step.r1 - step.r0), "chunk", tail_raw.device)
+    if tail_out.data_ptr() == tail_raw.data_ptr():
+        raise ValueError("tail_out must not be tail_raw")
+    _lib.check(_lib.lib().seist_stream_keep(_ref(step), tail_raw.data_ptr(), chunk.data_ptr() if step.r1 > step.r0 else None,
+                                            tail_out.data_ptr(), _s()), "seist_stream_keep")
+    return tail_out
+
+
+class StreamOutput(NamedTuple):
+    """What one call of a stream made final: probs (S, 3, m) of samples [t0, t0 + m); the picks (index int64 global, prob,
+    offsets (S + 1,)) and detection runs (pairs (E, 2) int64 global, offsets) that closed in the call, per station in
+    index order."""
+    t0: int
+    probs: torch.Tensor
+    ppk: tuple
+    spk: tuple
+    det: tuple
+
+
+class PickStream:
+    """The probability side of a stream: takes the final (S, 3, m) probabilities of a record in order, stretch after
+    stretch, and returns the picks and detection runs that closed (DESIGN §4.16).  A candidate is decided once the
+    sample after it is final; a cluster of candidates (consecutive gaps <= min_peak_dist) is resolved once its last
+    candidate c has c + min_peak_dist <= F - 2 (F: the final samples so far), so a pick waits for its cluster to close.
+    A run closes once the sample after its end is final.  `t0` is the global index of the first sample."""
+
+    def __init__(self, n_stations: int, device, min_peak_dist: int, ppk_threshold: float = 0.3, spk_threshold: float = 0.3,
+                 det_threshold: float = 0.5, t0: int = 0):
+        if min_peak_dist is None or int(min_peak_dist) <= 1:
+            raise ValueError(f"min_peak_dist must be > 1 samples, got {min_peak_dist}")
+        if int(n_stations) < 1:
+            raise ValueError(f"need at least one station, got {n_stations}")
+        self.S, self.device, self.mpd = int(n_stations), torch.device(device), int(min_peak_dist)
+        if self.device.type == "cuda" and self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.thr = (float(det_threshold), float(ppk_threshold), float(spk_threshold))
+        self.t0 = self.F = int(t0)
+        self.closed = False
+        self.look = torch.full((self.S, 3, 2), float("-inf"), device=self.device)      # the last two final samples
+        self.open = torch.full((self.S,), -1, dtype=torch.int64, device=self.device)   # start of each open run
+        self.pend = {1: None, 2: None}        # per pick channel: (work, capc, L, base) of the previous call
+        self.max_pend = {1: 0, 2: 0}
+        self.first_pend = {1: _I64_MAX, 2: _I64_MAX}
+
+    def push(self, probs: torch.Tensor):
+        """The next final stretch (S, 3, m), m >= 0 -> (ppk, spk, det) that closed."""
+        return self._step(probs, False)
+
+    def close(self, probs: torch.Tensor | None = None):
+        """The last stretch: every pending cluster and open run closes; sample F - 1 ends the record."""
+        if probs is None:
+            probs = torch.empty(self.S, 3, 0, device=self.device)
+        return self._step(probs, True)
+
+    def _step(self, probs: torch.Tensor, last: bool):
+        if self.closed:
+            raise RuntimeError("the stream is closed")
+        if not probs.is_cuda:
+            raise RuntimeError("PickStream has no CPU path: the probabilities must live on a CUDA device")
+        _dense(probs, (self.S, 3, None), "probabilities", self.device)
+        S, m = self.S, probs.shape[2]
+        f0, f1 = self.F, self.F + m
+        if last and f1 - self.t0 < 3:
+            raise ValueError(f"a record of {f1 - self.t0} samples is too short to pick")
+        lib, dev = _lib.lib(), self.device
+        parts = [self.look, probs] + ([torch.full((S, 3, 1), float("-inf"), device=dev)] if last else [])
+        ext = torch.cat(parts, 2)
+        L, g0 = ext.shape[2], f0 - 2
+        if L > _I32_MAX:
+            raise ValueError(f"a stretch of {m} samples is too long for one call")
+        staged = []
+        for ch in (1, 2):
+            prev = self.pend[ch]
+            base = min(g0, self.first_pend[ch])
+            if f1 - base >= _I32_MAX - 2:
+                raise RuntimeError(f"a cluster of candidates spans more than 2^31 samples (channel {ch})")
+            capc = self.max_pend[ch] + L // 2 + 1
+            nbytes = lib.seist_stream_peaks_work_bytes(S, capc, L)
+            work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            counts = torch.empty(S, dtype=torch.int64, device=dev)
+            info = torch.empty(2 * S, dtype=torch.int64, device=dev)
+            lim = _I64_MAX >> 1 if last else f1 - 2 - base
+            _lib.check(lib.seist_stream_peaks(ext.data_ptr(), S, 3, ch, L, max(1, 3 - (f0 - self.t0)), m, self.thr[ch], self.mpd, lim,
+                                              base, g0 - base, work.data_ptr(), capc,
+                                              prev[0].data_ptr() if prev else None, prev[1] if prev else 0, prev[2] if prev else 0,
+                                              base - prev[3] if prev else 0, self.max_pend[ch], counts.data_ptr(), info.data_ptr(),
+                                              _s()), "seist_stream_peaks")
+            staged.append((work, capc, base, _offsets(counts), info))
+        hi = m + 2 if last else m + 1
+        rbytes = lib.seist_runs_work_bytes(S, L)
+        rwork = torch.empty(rbytes, dtype=torch.uint8, device=dev)
+        rcounts = torch.empty(S, dtype=torch.int64, device=dev)
+        open_out = torch.empty(S, dtype=torch.int64, device=dev)
+        _lib.check(lib.seist_stream_runs(ext.data_ptr(), S, 3, 0, L, 2, hi, self.thr[0], self.open.data_ptr(), open_out.data_ptr(),
+                                         rwork.data_ptr(), rbytes, rcounts.data_ptr(), _s()), "seist_stream_runs")
+        roff = _offsets(rcounts)
+        tot = torch.cat([staged[0][3][-1:], staged[1][3][-1:], roff[-1:], staged[0][4], staged[1][4]]).tolist()   # the one host sync
+        out = []
+        for i, (ch, (work, capc, base, off, info)) in enumerate(zip((1, 2), staged)):
+            n = tot[i]
+            index = torch.empty(n, dtype=torch.int64, device=dev)
+            value = torch.empty(n, dtype=torch.float32, device=dev)
+            if n:
+                _lib.check(lib.seist_stream_peaks_fill(S, L, work.data_ptr(), capc, base, off.data_ptr(), index.data_ptr(),
+                                                       value.data_ptr(), _s()), "seist_stream_peaks_fill")
+            out.append((index, value, off))
+            o = 3 + 2 * S * i
+            self.max_pend[ch] = max(tot[o:o + S])
+            self.first_pend[ch] = min(tot[o + S:o + 2 * S])
+            self.pend[ch] = (work, capc, L, base)
+        pairs = torch.empty(tot[2], 2, dtype=torch.int64, device=dev)
+        _lib.check(lib.seist_stream_runs_fill(ext.data_ptr(), S, 3, 0, L, 2, hi, self.thr[0], g0, self.open.data_ptr(),
+                                              open_out.data_ptr(), rwork.data_ptr(), rbytes, roff.data_ptr(),
+                                              pairs.data_ptr() if pairs.numel() else None, _s()), "seist_stream_runs_fill")
+        self.open = open_out
+        self.look = ext[:, :, m:m + 2].clone()
+        self.F = f1
+        self.closed = last
+        return out[0], out[1], (pairs, roff)
+
+
+class ContinuousStream:
+    """A record annotated chunk by chunk (`ContinuousAnnotator.open_stream`).  `push(chunk)` takes (S, C, n) float32 on the
+    model's device, any n >= 0; `close()` ends the record.  Each returns a StreamOutput; concatenated, their probs equal
+    `annotate(record)` and their picks / runs `pick_phases` / `detect_events` of it (DESIGN §4.16).  Held between calls:
+    the last W raw samples, the partial sums of the samples not yet final, and the pending pick clusters and open runs."""
+
+    def __init__(self, ann: "ContinuousAnnotator", n_stations: int):
+        self.ann = ann
+        self.S, self.C = int(n_stations), ann.in_channels
+        self.device = next(ann.model.parameters()).device
+        W = ann.window
+        self.tail = [torch.zeros(self.S, self.C, W, device=self.device) for _ in range(2)]
+        self.carry = [torch.zeros(self.S, 3, W, device=self.device) for _ in range(2)]
+        self.R = self.F = self.k = 0
+        self.forwards = 0
+        self.picker = PickStream(self.S, self.device, ann.min_peak_dist, ann.thresholds["ppk"], ann.thresholds["spk"],
+                                 ann.thresholds["det"])
+
+    @property
+    def closed(self) -> bool:
+        return self.picker.closed
+
+    @torch.no_grad()
+    def push(self, chunk: torch.Tensor) -> StreamOutput:
+        if self.closed:
+            raise RuntimeError("push() after close()")
+        if not chunk.is_cuda:
+            raise RuntimeError("ContinuousStream has no CPU path: the chunk must live on the model's CUDA device")
+        if chunk.device != self.device:
+            raise RuntimeError(f"chunk on {chunk.device}, model on {self.device}")
+        if chunk.dtype != torch.float32 or chunk.dim() != 3 or chunk.shape[0] != self.S or chunk.shape[1] != self.C:
+            raise ValueError(f"expected a ({self.S}, {self.C}, n) float32 chunk, got {tuple(chunk.shape)} {chunk.dtype}")
+        if not chunk.is_contiguous():
+            raise ValueError("the chunk must be contiguous")
+        W, P = self.ann.window, self.ann.stride
+        r1 = self.R + chunk.shape[2]
+        k1 = (r1 - W) // P + 1 if r1 >= W else 0
+        return self._call(self.R, max(0, r1 - W), r1, k1 - self.k, -1, -1, chunk)
+
+    @torch.no_grad()
+    def close(self) -> StreamOutput:
+        if self.closed:
+            raise RuntimeError("close() after close()")
+        W, P, T = self.ann.window, self.ann.stride, self.R
+        if T < W:
+            raise ValueError(f"the record ({T} samples) is shorter than one window ({W})")
+        kr = (T - W) // P + 1
+        tail = T - W if (kr - 1) * P + W < T else -1
+        return self._call(T, T, T, 0, tail, kr, None)
+
+    def _call(self, r0, f1, r1, nk, tail, kr, chunk):
+        ann, S, W = self.ann, self.S, self.ann.window
+        step = stream_step(S, self.C, W, ann.stride, self.F, r0, f1, r1, self.k, nk, tail, kr, ann.norm_mode, ann.stack)
+        acc = torch.empty(S, 3, r1 - self.F, device=self.device)
+        nw = nk + (tail >= 0)
+        for j0 in range(0, S * nw, ann.batch):
+            stream_window_(ann.graph.x, step, self.tail[0], chunk, j0)
+            y = ann.graph.replay()
+            stream_stack_(acc, y, step, j0, self.carry[0])
+            self.forwards += 1
+        probs = torch.empty(S, 3, f1 - self.F, device=self.device)
+        stream_emit_(probs, self.carry[1], step, self.carry[0], acc)
+        stream_keep_(self.tail[1], step, self.tail[0], chunk)
+        self.tail.reverse()
+        self.carry.reverse()
+        t0 = self.F
+        self.R, self.F, self.k = r1, f1, self.k + nk
+        ppk, spk, det = self.picker.close(probs) if tail >= 0 or kr >= 0 else self.picker.push(probs)
+        return StreamOutput(t0, probs, ppk, spk, det)
+
+
 class ContinuousAnnotator:
     """`ann = ContinuousAnnotator(model, window=8192, stride=4096, batch=256, norm_mode="std", stack="mean")`
 
@@ -150,6 +406,8 @@ class ContinuousAnnotator:
     * `ann.pick_phases(probs, ppk_threshold, spk_threshold, min_peak_dist)` -> {"ppk": (index, prob, offsets), "spk": ...}
       with min_peak_dist in samples (> 1); `ann.split(picks["ppk"])` -> a list of (index, prob) per station.
     * `ann.detect_events(probs, det_threshold)` -> (pairs (E, 2), offsets (S + 1,)).
+    * `st = ann.open_stream(n_stations)`: the same, chunk by chunk (`st.push(chunk)`, `st.close()`, ContinuousStream);
+      thresholds and min_peak_dist are read here.
     Only the seist_*_dpk models (a [det, P, S] probability head) are supported."""
 
     def __init__(self, model, window: int = 8192, stride: int | None = None, batch: int = 256, norm_mode: str = "std",
@@ -211,6 +469,11 @@ class ContinuousAnnotator:
             y = self.graph.replay()
             stack_batch_(probs, y, self.window, self.stride, w0, self.stack)
         return stack_finish_(probs, self.window, self.stride, self.stack)
+
+    def open_stream(self, n_stations: int) -> ContinuousStream:
+        if self.min_peak_dist is None or int(self.min_peak_dist) <= 1:
+            raise ValueError(f"min_peak_dist must be > 1 samples, got {self.min_peak_dist}")
+        return ContinuousStream(self, n_stations)
 
     def pick_phases(self, probs: torch.Tensor, ppk_threshold: float | None = None, spk_threshold: float | None = None,
                     min_peak_dist: int | None = None):
