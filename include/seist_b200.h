@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 13
+#define SEIST_ABI_VERSION 14
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -327,6 +327,20 @@ int seist_runs_long(const float* prob, int32_t S, int32_t C, int32_t channel, in
                     int64_t work_bytes, int64_t* counts, void* stream);
 int seist_runs_long_fill(const float* prob, int32_t S, int32_t C, int32_t channel, int64_t T, float threshold, const void* work,
                          int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream);
+
+/* ---- picked events on continuous records (DESIGN §4.17): P-anchored windows for the non-dpk heads -------------------
+   The reference cuts one event window with `_cut_window` and 0 <= p_position_ratio <= 1 (training/preprocess.py:172-203):
+   W samples with the first P pick at sample anchor = int(W * p_position_ratio) (computed by the caller), zero-filled
+   outside the trace, then `_normalize` (:224-242).  record (S, C, T) fp32, 1 <= T < 2^31; index (M,) int64 P sample
+   indices (may be null when M = 0) and offsets (S + 1,) int64 the CSR of seist_peaks_long_fill (station s holds events offsets[s] .. offsets[s+1]).
+   seist_event_windows = for d < n_dst (<= 4), x[d] (B, C, W) = the input of events e0 .. e0 + B - 1: row (b, c) is
+                         record[s, c, p - anchor + i], i < W, with 0.0f outside [0, T), normalised as seist_normalize (mode
+                         0 none, 1 std, 2 max; W <= 49152); p = index[e0 + b], s the last station with offsets[s] <= e0 + b
+                         (a bounded search: always in [0, S)).  Events >= M and picks outside [0, T) give zero rows (the
+                         reference's slicing would wrap around there).  Offsets are never read back to the host. */
+int seist_event_windows(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* index, int64_t M,
+                        const int64_t* offsets, int64_t e0, int32_t B, int32_t W, int32_t anchor, int32_t mode, float* const* x,
+                        int32_t n_dst, void* stream);
 
 /* ---- continuous records streamed chunk by chunk (DESIGN §4.16) -------------------------------------------------------
    One call of a stream (a push of n samples per station, or the close) as global int64 sample counts from the start of the

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 13
+ABI_VERSION = 14
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -169,6 +169,9 @@ def lib():
     L.seist_window_batch.restype = C.c_int
     L.seist_window_batch.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32,
                                      C.c_int32, C.c_void_p, C.c_void_p]
+    L.seist_event_windows.restype = C.c_int
+    L.seist_event_windows.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     L.seist_stack_batch.restype = C.c_int
     L.seist_stack_batch.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_void_p]
@@ -244,7 +247,7 @@ EXPORTS = [
     "seist_pick_phase", "seist_detect_event", "seist_pick_counters", "seist_det_counters",
     "seist_normalize", "seist_dpk_labels", "seist_ce_fwd", "seist_ce_bwd",
     "seist_augment", "seist_sizeof_aug", "seist_aug_recipe_bytes",
-    "seist_window_batch", "seist_stack_batch", "seist_stack_finish", "seist_peaks_work_bytes", "seist_peaks_long",
+    "seist_window_batch", "seist_event_windows", "seist_stack_batch", "seist_stack_finish", "seist_peaks_work_bytes", "seist_peaks_long",
     "seist_peaks_long_fill", "seist_runs_work_bytes", "seist_runs_long", "seist_runs_long_fill",
     "seist_sizeof_stream_step", "seist_stream_window", "seist_stream_stack", "seist_stream_emit", "seist_stream_keep",
     "seist_stream_peaks_work_bytes", "seist_stream_peaks", "seist_stream_peaks_fill", "seist_stream_runs", "seist_stream_runs_fill",

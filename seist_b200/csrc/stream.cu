@@ -54,6 +54,54 @@ __global__ void __launch_bounds__(PR_NT) window_batch_kernel(const float* __rest
   pr_normalize_row(wb_row, dst, win.W, mode);
 }
 
+// ---- P-anchored event windows (DESIGN §4.17) ----------------------------------------------------------------------
+// `_cut_window` with 0 <= p_position_ratio <= 1 (training/preprocess.py:172-203) then `_normalize` of every P pick of a
+// CSR pick list.  x_d (B, C, W), d < n_dst: row (b, c) = normalised record[s, c, p - a + i], i < W, 0.0f where p - a + i
+// falls outside [0, T); p = index[e0 + b], s the station whose offsets range holds event e0 + b.  Events >= M and picks
+// outside [0, T) give zero rows.
+constexpr int EW_MAX_DST = 4;
+struct EventDst {
+  float* x[EW_MAX_DST];
+};
+
+__global__ void __launch_bounds__(PR_NT) event_windows_kernel(const float* __restrict__ rec, int S, int C, int T,
+                                                              const long long* __restrict__ index,
+                                                              const long long* __restrict__ offsets, long long M, long long e0,
+                                                              int W, int a, int mode, EventDst dst, int n_dst) {
+  extern __shared__ float ew_row[];                 // [W]: the zero-filled record slice, normalised in place
+  const int b = blockIdx.x / C, c = blockIdx.x % C;
+  const long long e = e0 + b;
+  const size_t row = (size_t)blockIdx.x * W;
+  const long long p = e < M ? index[e] : -1;
+  if (p < 0 || p >= T) {
+#pragma unroll
+    for (int d = 0; d < EW_MAX_DST; ++d)           // unrolled: a runtime index into dst would put it on the stack
+      if (d < n_dst)
+        for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = 0.f;
+    return;
+  }
+  // the last station s with offsets[s] <= e (empty stations before it share its start); always in [0, S), so
+  // malformed offsets pick a wrong station but never an out-of-range one
+  int lo = 0, hi = S - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (offsets[mid] <= e) lo = mid; else hi = mid - 1;
+  }
+  const float* src = rec + ((size_t)lo * C + c) * T;
+  const long long t0 = p - a;
+  for (int i = threadIdx.x; i < W; i += PR_NT) {
+    const long long t = t0 + i;
+    ew_row[i] = t >= 0 && t < T ? src[t] : 0.f;
+  }
+  __syncthreads();
+  pr_normalize_row(ew_row, ew_row, W, mode);
+  // each thread stores the elements it normalised itself: no barrier needed
+#pragma unroll
+  for (int d = 0; d < EW_MAX_DST; ++d)
+    if (d < n_dst)
+      for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = ew_row[i];
+}
+
 // ---- stacking -----------------------------------------------------------------------------------------------------
 // Gather: the thread of probs[s, c, t] adds (maxes) the batch's covering windows of t in ascending window order; the
 // first covering window of t overall starts the accumulator (0.0f + v for the mean, fmaxf(-inf, v) for the max).
@@ -644,6 +692,31 @@ int seist_window_batch(const float* record, int32_t S, int32_t C, int64_t T, int
                                                                                            mode, x);
   note_launch();
   return check_launch("window_batch");
+}
+
+int seist_event_windows(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* index, int64_t M,
+                        const int64_t* offsets, int64_t e0, int32_t B, int32_t W, int32_t anchor, int32_t mode, float* const* x,
+                        int32_t n_dst, void* stream) {
+  bool ok = record && (index || M == 0) && offsets && x && S > 0 && C > 0 && T >= 1 && T <= INT32_MAX && M >= 0 && e0 >= 0 && B > 0 &&
+            (long long)B * C <= INT32_MAX && W >= 1 && W <= 49152 && anchor >= 0 && anchor <= W && mode >= 0 && mode <= 2 &&
+            n_dst >= 1 && n_dst <= EW_MAX_DST;
+  EventDst dst{};
+  for (int d = 0; ok && d < n_dst; ++d) ok = (dst.x[d] = x[d]) != nullptr;
+  if (!ok) {
+    set_error("event_windows: bad arguments (1 <= T < 2^31, 1 <= W <= 49152, 0 <= anchor <= W, M >= 0, e0 >= 0, B > 0, "
+              "mode 0 none, 1 std, 2 max, 1 to 4 non-null destinations)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(event_windows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  event_windows_kernel<<<(unsigned)((long long)B * C), PR_NT, smem, (cudaStream_t)stream>>>(
+      record, S, C, (int)T, (const long long*)index, (const long long*)offsets, M, e0, W, anchor, mode, dst, n_dst);
+  note_launch();
+  return check_launch("event_windows");
 }
 
 int seist_stack_batch(const float* y, int32_t S, int64_t T, int32_t W, int32_t P, int64_t w0, int32_t B, int32_t mode, float* probs,
