@@ -1,7 +1,8 @@
-"""CPU interpreter of seist_b200 plans.  TEST INFRASTRUCTURE ONLY (never imported by the product).
+"""Interpreter of seist_b200 plans.  TEST INFRASTRUCTURE ONLY (never imported by the product).
 
-Executes the *semantics* of every SeistOp kind (include/seist_b200.h) with plain torch CPU ops on the
-plan's own buffers, so that
+Executes the *semantics* of every SeistOp kind (include/seist_b200.h) with plain torch ops on the plan's own
+buffers, on the plan's device (a CPU plan on the CPU, a CUDA plan on the GPU) in the arithmetic `dtype` names,
+so that
   (1) the plan compiler (seist_b200/plan.py: forward tape, derived backward, accumulate flags,
       BatchNorm-backward coefficient algebra, chained-BN folding) is checked end-to-end against the
       pinned oracle (oracle/seist_ref.py) without a GPU, and
@@ -56,6 +57,7 @@ class Interp:
     def __init__(self, plan: Plan, dtype=torch.float32):
         self.p = plan
         self.dt = dtype
+        self.dev = plan.flat.P.device       # the plan's own device: a CUDA plan is interpreted there
 
     # ---- BatchNorm coefficient algebra (mirrors csrc/common.cuh) ---------------------------------
     def _stats(self, e):
@@ -164,15 +166,15 @@ class Interp:
         """delta(n) * D(n,c,l) multiplying conv+bias, and alpha(n)."""
         N, C, L = f.N, f.Cout, f.L_out
         seed = int(self.p.step_seed.item())
-        fac = torch.ones(N, C, L, dtype=self.dt)
+        fac = torch.ones(N, C, L, dtype=self.dt, device=self.dev)
         if f.p_elem > 0:
             idx = np.arange(N * C * L, dtype=np.uint64)
-            fac = fac * keep_mask(f.p_elem, seed, f.seed_elem, idx).view(N, C, L).to(self.dt)
+            fac = fac * keep_mask(f.p_elem, seed, f.seed_elem, idx).view(N, C, L).to(self.dev, self.dt)
         if f.p_path > 0:
-            fac = fac * keep_mask(f.p_path, seed, f.seed_path, np.arange(N, dtype=np.uint64)).view(N, 1, 1).to(self.dt)
-        alpha = torch.ones(N, 1, 1, dtype=self.dt)
+            fac = fac * keep_mask(f.p_path, seed, f.seed_path, np.arange(N, dtype=np.uint64)).view(N, 1, 1).to(self.dev, self.dt)
+        alpha = torch.ones(N, 1, 1, dtype=self.dt, device=self.dev)
         if f.p_alpha > 0:
-            alpha = keep_mask(f.p_alpha, seed, f.seed_alpha, np.arange(N, dtype=np.uint64)).view(N, 1, 1).to(self.dt)
+            alpha = keep_mask(f.p_alpha, seed, f.seed_alpha, np.arange(N, dtype=np.uint64)).view(N, 1, 1).to(self.dev, self.dt)
         return fac, alpha
 
     def _W(self, f: Op):
@@ -223,7 +225,7 @@ class Interp:
         if f.p_attn > 0:
             Lk = kh.shape[-1]
             idx = np.arange(N * H * Lq * Lk, dtype=np.uint64)
-            a = a * keep_mask(f.p_attn, int(self.p.step_seed.item()), f.seed_attn, idx).view(N, H, Lq, Lk).to(self.dt)
+            a = a * keep_mask(f.p_attn, int(self.p.step_seed.item()), f.seed_attn, idx).view(N, H, Lq, Lk).to(self.dev, self.dt)
         o = (a @ vh.transpose(-1, -2)).transpose(-1, -2).reshape(N, C, Lq)
         return o, lse
 
@@ -295,7 +297,7 @@ class Interp:
     def out_grad(self, f: Op) -> torch.Tensor:
         o = f.out
         sl = slice(o.c0, o.c0 + o.C)
-        g = torch.zeros(f.N, o.C, o.buf.L, dtype=self.dt)
+        g = torch.zeros(f.N, o.C, o.buf.L, dtype=self.dt, device=self.dev)
         if o.buf.dxd is not None:
             g = g + o.buf.dxd[:, sl].to(self.dt)
         if o.bn >= 0 and o.buf.du is not None:
