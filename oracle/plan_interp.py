@@ -53,6 +53,23 @@ def keep_mask(p: float, step_seed: int, stream: int, idx: np.ndarray) -> torch.T
     return torch.from_numpy(keep.astype(np.float32)) / np.float32(1.0 - np.float32(p))
 
 
+def upsample_linear(X: torch.Tensor, size: int) -> torch.Tensor:
+    """F.interpolate(X, size=size, mode="linear") (align_corners=False) with the source coordinates the fp32 model
+    computes, whatever the dtype of X: ratio = fp32(L_src) / fp32(size) and src = ratio * (p + 0.5) - 0.5 rounded to fp32
+    once (the fused multiply-add of csrc/conv_common.cuh::upsample_coords).  Where size / L_src is not a power of two,
+    the fp32 coordinate of a sample near the end of a row is ~L_src * 2^-24 off the exact one (1e-4 at L_src = 1501),
+    which shifts its interpolation weights by as much; the coordinates are part of what the op computes, so the
+    interpreter takes them from the fp32 model and only the blend runs in X's dtype."""
+    Ls = X.shape[-1]
+    ratio = (torch.tensor(Ls, dtype=torch.float32) / torch.tensor(size, dtype=torch.float32)).item()
+    p = torch.arange(size, dtype=torch.float64, device=X.device)
+    src = (ratio * (p + 0.5) - 0.5).float().double().clamp_min(0)     # exact in float64, then one fp32 rounding
+    i0 = src.long().clamp_max(Ls - 1)
+    i1 = (i0 + 1).clamp_max(Ls - 1)
+    lam = (src - i0).clamp(0, 1).to(X.dtype)
+    return X[..., i0] * (1 - lam) + X[..., i1] * lam
+
+
 class Interp:
     def __init__(self, plan: Plan, dtype=torch.float32):
         self.p = plan
@@ -157,7 +174,7 @@ class Interp:
         if f.pool > 1:
             X = F.avg_pool1d(X, f.pool, ceil_mode=True) + F.max_pool1d(X, f.pool, ceil_mode=True)
         elif f.up_src_L > 0:
-            X = F.interpolate(X, size=f.L_in, mode="linear")
+            X = upsample_linear(X, f.L_in)
         pr = (f.L_out - 1) * f.stride + f.k - f.L_in - f.pad_left
         X = F.pad(X, (f.pad_left, pr))
         return F.conv1d(X, W, None, stride=f.stride, groups=f.groups)
