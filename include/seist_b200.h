@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 14
+#define SEIST_ABI_VERSION 15
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -393,6 +393,14 @@ int seist_stream_stack(const SeistStreamStep* step, const float* y, int64_t j0, 
 int seist_stream_emit(const SeistStreamStep* step, const float* carry, const float* acc, float* probs, float* carry_out,
                       void* stream);
 int seist_stream_keep(const SeistStreamStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream);
+/* Raw history of a characterised stream (DESIGN §4.18): held (S, C, n_held) holds the global samples
+   [h0_held, h0_held + n_held) of every row, chunk (S, C, n) the n samples after them.  out (S, C, n_out) = the samples
+   [h0_out, h0_held + n_held + n), n_out = h0_held + n_held + n - h0_out, rows packed at stride n_out; out_capacity (floats)
+   >= S * C * n_out and out overlaps neither input.  Needs 0 <= h0_held <= h0_out, 0 <= n_out < 2^31, S * C <= 65535; each
+   retained sample is read and written once, and n_out = 0 launches nothing (out may then be null).  seist_event_windows cuts from out with
+   T = n_out and the pick indices rebased by -h0_out. */
+int seist_stream_history(const float* held, int64_t h0_held, int64_t n_held, const float* chunk, int64_t n, int64_t h0_out,
+                         int32_t S, int32_t C, float* out, int64_t out_capacity, void* stream);
 int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L);
 int seist_stream_peaks(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float mph,
                        int32_t min_peak_dist, int64_t lim, int64_t base, int32_t ishift, void* work, int32_t capc,

@@ -467,6 +467,22 @@ __global__ void __launch_bounds__(ST_NT) stream_keep_kernel(SeistStreamStep p, c
   if (i < keep) tail_out[(size_t)blockIdx.y * p.W + i] = ss_raw(p, tail, chunk, s, c, p.r1 - keep + i);
 }
 
+// ---- raw history of a characterised stream (DESIGN §4.18) ----------------------------------------------------------
+// out (S, C, n_out), row (s, c) = samples [h0_out, h0_out + n_out) of held (S, C, n_held, base h0_held) followed by the
+// chunk (S, C, n); j = h0_out - h0_held + i indexes held ++ chunk.  Every read is range-checked (0.0f outside).
+__global__ void __launch_bounds__(ST_NT) stream_history_kernel(const float* __restrict__ held, long long n_held,
+                                                               const float* __restrict__ chunk, long long n, long long shift,
+                                                               long long n_out, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * ST_NT + threadIdx.x;
+  if (i >= n_out) return;
+  const size_t row = blockIdx.y;
+  const long long j = shift + i;
+  float v = 0.f;
+  if (j >= 0 && j < n_held) v = held[row * (size_t)n_held + (size_t)j];
+  else if (j >= n_held && j - n_held < n) v = chunk[row * (size_t)n + (size_t)(j - n_held)];
+  out[row * (size_t)n_out + (size_t)i] = v;
+}
+
 // stack_batch_kernel for the call's windows j0 .. j0 + nb - 1 into acc ([f0, r1)).  A sample that is not new continues
 // from acc when an earlier batch of the call covered it (the station's part of the batch starts after the call's first
 // window: the window before it covers t), else from carry ([f0, r0), earlier calls)
@@ -898,6 +914,23 @@ int seist_stream_keep(const SeistStreamStep* step, const float* tail_raw, const 
       *step, tail_raw, chunk, tail_out);
   note_launch();
   return check_launch("stream_keep");
+}
+
+int seist_stream_history(const float* held, int64_t h0_held, int64_t n_held, const float* chunk, int64_t n, int64_t h0_out,
+                         int32_t S, int32_t C, float* out, int64_t out_capacity, void* stream) {
+  const long long n_out = h0_held + n_held + n - h0_out;
+  if (S <= 0 || C <= 0 || (long long)S * C > 65535 || h0_held < 0 || n_held < 0 || n < 0 || h0_out < h0_held || n_out < 0 ||
+      n_out > INT32_MAX || (n_held > 0 && !held) || (n > 0 && !chunk) || out_capacity < (long long)S * C * n_out ||
+      (n_out > 0 && (!out || out == held || out == chunk))) {
+    set_error("stream_history: bad arguments (0 <= h0_held <= h0_out <= h0_held + n_held + n, output length < 2^31, "
+              "S * C <= 65535, out_capacity >= S * C * output length, out distinct from held and chunk)");
+    return -1;
+  }
+  if (n_out == 0) return 0;
+  stream_history_kernel<<<dim3((unsigned)((n_out + ST_NT - 1) / ST_NT), (unsigned)(S * C)), ST_NT, 0, (cudaStream_t)stream>>>(
+      held, n_held, chunk, n, h0_out - h0_held, n_out, out);
+  note_launch();
+  return check_launch("stream_history");
 }
 
 int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L) {

@@ -7,17 +7,19 @@ zero-filling what falls outside the trace, and `_normalize` (:224-242) normalise
 picks of a whole record, as the CSR `ContinuousAnnotator.pick_phases(...)["ppk"]` returns them, are cut straight into the
 static inputs of the models' captured eval plans (`InferenceGraph`) by one kernel launch per batch of events
 (`seist_event_windows`, csrc/stream.cu), and the outputs come back aligned index for index with the pick list.  The numpy
-restatement of the cut is `oracle/event_ref.py`.  There is no CPU path.
+restatement of the cut is `oracle/event_ref.py`.  `EventCharacterizer.open_stream` does the same for the P picks of a
+record streamed chunk by chunk, in the call that emits them (DESIGN §4.18).  There is no CPU path.
 """
 from __future__ import annotations
 
 import ctypes
+from typing import NamedTuple
 
 import torch
 
 from . import _lib
 from .infer import InferenceGraph
-from .stream import _MODES, _dense, _s
+from .stream import _I32_MAX, _MODES, ContinuousAnnotator, StreamOutput, _dense, _s
 
 MAX_MODELS = 4              # destinations of one seist_event_windows launch
 MAX_WINDOW = 49152          # a row of the window is staged in shared memory
@@ -128,7 +130,9 @@ class EventCharacterizer:
         if T >= 2 ** 31:
             raise ValueError(f"record length {T} must stay below 2^31 samples")
         _check_picks(index, offsets, S, self.device)
-        record = record.contiguous()
+        return self._run(record.contiguous(), index, offsets)
+
+    def _run(self, record: torch.Tensor, index: torch.Tensor, offsets: torch.Tensor) -> dict:
         M = index.numel()
         out = {name: torch.empty((M,) if self.heads[name] == "reg" else (M, g.y.shape[1]), dtype=torch.float32, device=self.device)
                for name, g in self.graphs.items()}
@@ -140,3 +144,97 @@ class EventCharacterizer:
                 y = g.replay()
                 out[name][e0:e0 + n] = y[:n, 0] if self.heads[name] == "reg" else y[:n]
         return out
+
+    def open_stream(self, annotator: ContinuousAnnotator, n_stations: int) -> "CharacterizedStream":
+        """A record picked chunk by chunk by `annotator` (a dpk ContinuousAnnotator, thresholds and min_peak_dist set),
+        every P pick characterised in the call that emits it (DESIGN §4.18)."""
+        return CharacterizedStream(self, annotator, n_stations)
+
+
+def stream_history_(out: torch.Tensor, held: torch.Tensor, h0_held: int, chunk: torch.Tensor | None, h0_out: int) -> torch.Tensor:
+    """The raw samples [h0_out, h0_held + held.shape[2] + n) of every row, from held (S, C, n_held: samples h0_held ..)
+    followed by chunk (S, C, n), written packed into the flat float32 buffer out -> the (S, C, n_out) view of it."""
+    _dense(held, (None, None, None), "held samples")
+    S, C, n_held = held.shape
+    n = 0 if chunk is None else chunk.shape[2]
+    if chunk is not None:
+        _dense(chunk, (S, C, None), "chunk", held.device)
+    _dense(out, (None,), "history buffer", held.device)
+    n_out = h0_held + n_held + n - h0_out
+    if not (0 <= h0_held <= h0_out and 0 <= n_out <= _I32_MAX and S * C * n_out <= out.numel()):
+        raise ValueError(f"need 0 <= h0_held <= h0_out, an output of 0 .. 2^31 - 1 samples and a buffer of S * C * n_out floats, "
+                         f"got h0_held {h0_held}, h0_out {h0_out}, n_out {n_out}, buffer {out.numel()}")
+    _lib.check(_lib.lib().seist_stream_history(held.data_ptr() if n_held else None, h0_held, n_held, chunk.data_ptr() if n else None, n,
+                                               h0_out, S, C, out.data_ptr(), out.numel(), _s()), "seist_stream_history")
+    return out[:S * C * n_out].view(S, C, n_out)
+
+
+class CharacterizedOutput(NamedTuple):
+    """One call of a CharacterizedStream: the stream's StreamOutput and {name: outputs} for its P picks, row i for pick i
+    of `out.ppk` ((m, classes) probabilities of a classification model, (m,) of a regression model)."""
+    out: StreamOutput
+    events: dict
+
+
+class CharacterizedStream:
+    """`EventCharacterizer.open_stream(annotator, n_stations)`: `push(chunk (S, C, n))` for any n >= 0, then `close()`, each
+    -> CharacterizedOutput.  Concatenated per station, the events equal `ch(record, annotator.pick_phases(
+    annotator.annotate(record))["ppk"])` bit for bit, and each comes out in the call that emits its pick (DESIGN §4.18).
+    Besides the ContinuousStream's state it holds the raw samples [h0, R) in one of two device buffers: h0 is the retention
+    bound max(0, min(first pending P candidate, F - 1) - anchor) of the call before the last non-empty push, below which
+    no pick emitted since then starts its window.  `held_samples` = R - h0."""
+
+    def __init__(self, ch: EventCharacterizer, ann: ContinuousAnnotator, n_stations: int):
+        dev = next(ann.model.parameters()).device
+        if dev != ch.device:
+            raise ValueError(f"the annotator's model is on {dev}, the characteriser's models on {ch.device}")
+        if ann.in_channels != ch.in_channels:
+            raise ValueError(f"the annotator takes {ann.in_channels} channels, the characteriser's models {ch.in_channels}")
+        if ch.window - ch.anchor > ann.window:
+            raise ValueError(f"the characteriser's window reaches {ch.window - ch.anchor} samples past the pick, more than the "
+                             f"annotator's window ({ann.window}): a pick's event window would not be pushed yet when it closes")
+        self.ch = ch
+        self.stream = ann.open_stream(n_stations)
+        self.S, self.C, self.device = self.stream.S, self.stream.C, self.stream.device
+        self.buf = [torch.empty(0, device=self.device), torch.empty(0, device=self.device)]
+        self.history = self.buf[0].view(self.S, self.C, 0)
+        self.h0 = self.R = 0
+        self.keep = 0            # the retention bound after the last call
+
+    @property
+    def closed(self) -> bool:
+        return self.stream.closed
+
+    @property
+    def forwards(self) -> int:
+        return self.stream.forwards
+
+    @property
+    def held_samples(self) -> int:
+        return self.R - self.h0
+
+    @torch.no_grad()
+    def push(self, chunk: torch.Tensor) -> CharacterizedOutput:
+        n = chunk.shape[2] if isinstance(chunk, torch.Tensor) and chunk.dim() == 3 else 0
+        if not self.closed and self.R + n - self.keep > _I32_MAX:
+            raise ValueError(f"the history would hold {self.R + n - self.keep} samples per row, more than 2^31 - 1")
+        out = self.stream.push(chunk)              # validates the chunk before any launch
+        if n:
+            need = self.S * self.C * (self.R + n - self.keep)
+            if self.buf[1].numel() < need:
+                self.buf[1] = torch.empty(max(need, 2 * self.buf[1].numel()), device=self.device)
+            self.history = stream_history_(self.buf[1], self.history, self.h0, chunk, self.keep)
+            self.buf.reverse()
+            self.h0, self.R = self.keep, self.R + n
+        return self._finish(out)
+
+    @torch.no_grad()
+    def close(self) -> CharacterizedOutput:
+        return self._finish(self.stream.close())
+
+    def _finish(self, out: StreamOutput) -> CharacterizedOutput:
+        pk = self.stream.picker
+        self.keep = max(self.keep, min(pk.first_pend[1], pk.F - 1) - self.ch.anchor)
+        index, _, offsets = out.ppk
+        rel = index - self.h0 if index.numel() else index
+        return CharacterizedOutput(out, self.ch._run(self.history, rel, offsets))
