@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 15
+#define SEIST_ABI_VERSION 16
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -413,6 +413,68 @@ int seist_stream_runs(const float* ext, int32_t S, int32_t C, int32_t channel, i
 int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi,
                            float threshold, int64_t g0, const int64_t* open_in, int64_t* open_out, const void* work,
                            int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream);
+
+/* ---- ragged streams: stations that advance at different rates (DESIGN §4.19) -----------------------------------------
+   One call of a ragged stream is SeistStreamStep per station: every per-station count is a device int64 array of S
+   entries (f0, r0, f1, r1, k0, nk, tail, kr as in SeistStreamStep), and four exclusive prefix arrays of S + 1 entries pack
+   the call's data back to back:
+     win_off   the call's windows, nk[s] + (tail[s] >= 0); call window j belongs to the last s with win_off[s] <= j and is
+               that station's window j - win_off[s] (the tail one last).
+     chunk_off the new samples: chunk holds station s as a (C, r1[s] - r0[s]) block at C * chunk_off[s].
+     acc_off   the partial sums: acc holds station s as a (3, r1[s] - f0[s]) block at 3 * acc_off[s].
+     out_off   the final probabilities: probs holds station s as a (3, f1[s] - f0[s]) block at 3 * out_off[s].
+   tail_raw / tail_out (S, C, W) and carry / carry_out (S, 3, W) are per station as in SeistStreamStep.  The host-side
+   totals n_win (= win_off[S]) and max_len (= max over s of r1[s] - f0[s]) size the grids; the arrays are never read back.
+   Every device read of raw samples, partial sums and carries is range-checked against the station's own counts.
+   seist_ragged_window = seist_stream_window for the call's windows j0 .. j0 + B - 1 (zero rows from n_win on).
+   seist_ragged_stack  = seist_stream_stack of those windows' outputs, per station; s0 .. s1 are the stations of windows
+                         j0 .. min(j0 + B, n_win) - 1 (the host knows win_off).  Call with j0 = 0, B, 2B, ... in order.
+   seist_ragged_emit   = probs and carry_out; seist_ragged_keep = tail_out (the last min(W, r1[s]) raw samples).
+   Picking a ragged stream: ext holds row s as a (C, L_s) block at C * ext_off[s], L_s = ext_off[s + 1] - ext_off[s]:
+   the two samples before the stretch, the stretch of m_s samples and at the close one -inf sentinel.
+   seist_ragged_ext    = ext from look (S, C, 2) and the stretches (probs packed at C * prob_off[s], (C, m_s)), every
+                         sample past them -inf (the sentinel when L_s = m_s + 3), plus look_out (S, C, 2) = ext samples
+                         m_s, m_s + 1 of each row.
+   seist_ragged_peaks  = seist_stream_peaks with lo, hi, lim, base, ishift (= g0 - base) and delta per row (device int64
+                         arrays); lo is raised to 1 and hi lowered to L_s - 2 in the kernels.  max_span >= max(hi - lo + 1)
+                         and max_L = max L_s size the grids; work: seist_stream_peaks_work_bytes(S, capc, max_L).
+                         seist_ragged_peaks_fill writes the picks (global index = base[s] + offset).
+   seist_ragged_runs   = seist_stream_runs with lo, hi and g0 per row (hi lowered to L_s - 1); work:
+                         seist_runs_work_bytes(S, max_L). */
+typedef struct SeistRaggedStep {
+  const int64_t *f0, *r0, *f1, *r1, *k0, *nk, *tail, *kr;   /* (S,) each */
+  const int64_t *win_off, *chunk_off, *acc_off, *out_off;    /* (S + 1,) each */
+  int64_t n_win;       /* win_off[S] */
+  int64_t max_len;     /* max over s of r1[s] - f0[s] */
+  int32_t S, C, W, P;
+  int32_t norm_mode;   /* 0 none, 1 std, 2 max */
+  int32_t stack_mode;  /* 0 mean, 1 max */
+} SeistRaggedStep;
+
+uint64_t seist_sizeof_ragged_step(void);
+int seist_ragged_window(const SeistRaggedStep* step, const float* tail_raw, const float* chunk, int64_t j0, int32_t B, float* x,
+                        void* stream);
+int seist_ragged_stack(const SeistRaggedStep* step, const float* y, int64_t j0, int32_t B, int32_t s0, int32_t s1,
+                       const float* carry, float* acc, void* stream);
+int seist_ragged_emit(const SeistRaggedStep* step, const float* carry, const float* acc, float* probs, float* carry_out,
+                      void* stream);
+int seist_ragged_keep(const SeistRaggedStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream);
+int seist_ragged_ext(const float* look, const float* probs, const int64_t* prob_off, const int64_t* ext_off, int32_t S, int32_t C,
+                     int64_t max_L, float* ext, float* look_out, void* stream);
+int seist_ragged_peaks(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
+                       const int64_t* lo, const int64_t* hi, int64_t max_span, float mph, int32_t min_peak_dist,
+                       const int64_t* lim, const int64_t* base, const int64_t* ishift, void* work, int32_t capc,
+                       const void* prev, int32_t prev_capc, int64_t prev_L, const int64_t* delta, int32_t max_pend,
+                       int64_t* counts, int64_t* info, void* stream);
+int seist_ragged_peaks_fill(int32_t S, int64_t max_L, const void* work, int32_t capc, const int64_t* base, const int64_t* offsets,
+                            int64_t* index, float* value, void* stream);
+int seist_ragged_runs(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
+                      const int64_t* lo, const int64_t* hi, int64_t max_span, float threshold, const int64_t* open_in,
+                      int64_t* open_out, void* work, int64_t work_bytes, int64_t* counts, void* stream);
+int seist_ragged_runs_fill(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
+                           const int64_t* lo, const int64_t* hi, int64_t max_span, float threshold, const int64_t* g0,
+                           const int64_t* open_in, int64_t* open_out, const void* work, int64_t work_bytes,
+                           const int64_t* offsets, int64_t* pairs, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 15
+ABI_VERSION = 16
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -84,6 +84,17 @@ class SeistStreamStep(C.Structure):
         ("k0", C.c_int64), ("tail", C.c_int64), ("kr", C.c_int64),
         ("S", C.c_int32), ("C", C.c_int32), ("W", C.c_int32), ("P", C.c_int32),
         ("nk", C.c_int32), ("norm_mode", C.c_int32), ("stack_mode", C.c_int32), ("pad_", C.c_int32),
+    ]
+
+
+class SeistRaggedStep(C.Structure):
+    _fields_ = [
+        ("f0", C.c_void_p), ("r0", C.c_void_p), ("f1", C.c_void_p), ("r1", C.c_void_p),
+        ("k0", C.c_void_p), ("nk", C.c_void_p), ("tail", C.c_void_p), ("kr", C.c_void_p),
+        ("win_off", C.c_void_p), ("chunk_off", C.c_void_p), ("acc_off", C.c_void_p), ("out_off", C.c_void_p),
+        ("n_win", C.c_int64), ("max_len", C.c_int64),
+        ("S", C.c_int32), ("C", C.c_int32), ("W", C.c_int32), ("P", C.c_int32),
+        ("norm_mode", C.c_int32), ("stack_mode", C.c_int32),
     ]
 
 
@@ -222,6 +233,27 @@ def lib():
     L.seist_stream_runs_fill.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
+    rstep = C.POINTER(SeistRaggedStep)
+    P, I32, I64, F32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
+    L.seist_sizeof_ragged_step.restype = C.c_uint64
+    L.seist_ragged_window.restype = C.c_int
+    L.seist_ragged_window.argtypes = [rstep, P, P, I64, I32, P, P]
+    L.seist_ragged_stack.restype = C.c_int
+    L.seist_ragged_stack.argtypes = [rstep, P, I64, I32, I32, I32, P, P, P]
+    L.seist_ragged_emit.restype = C.c_int
+    L.seist_ragged_emit.argtypes = [rstep, P, P, P, P, P]
+    L.seist_ragged_keep.restype = C.c_int
+    L.seist_ragged_keep.argtypes = [rstep, P, P, P, P]
+    L.seist_ragged_ext.restype = C.c_int
+    L.seist_ragged_ext.argtypes = [P, P, P, P, I32, I32, I64, P, P, P]
+    L.seist_ragged_peaks.restype = C.c_int
+    L.seist_ragged_peaks.argtypes = [P, P, I32, I32, I32, I64, P, P, I64, F32, I32, P, P, P, P, I32, P, I32, I64, P, I32, P, P, P]
+    L.seist_ragged_peaks_fill.restype = C.c_int
+    L.seist_ragged_peaks_fill.argtypes = [I32, I64, P, I32, P, P, P, P, P]
+    L.seist_ragged_runs.restype = C.c_int
+    L.seist_ragged_runs.argtypes = [P, P, I32, I32, I32, I64, P, P, I64, F32, P, P, P, I64, P, P]
+    L.seist_ragged_runs_fill.restype = C.c_int
+    L.seist_ragged_runs_fill.argtypes = [P, P, I32, I32, I32, I64, P, P, I64, F32, P, P, P, P, I64, P, P, P]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -239,6 +271,8 @@ def lib():
         raise RuntimeError(f"seist_b200: SeistAugCfg layout mismatch {L.seist_sizeof_aug()} vs {C.sizeof(SeistAugCfg)}")
     if L.seist_sizeof_stream_step() != C.sizeof(SeistStreamStep):
         raise RuntimeError(f"seist_b200: SeistStreamStep layout mismatch {L.seist_sizeof_stream_step()} vs {C.sizeof(SeistStreamStep)}")
+    if L.seist_sizeof_ragged_step() != C.sizeof(SeistRaggedStep):
+        raise RuntimeError(f"seist_b200: SeistRaggedStep layout mismatch {L.seist_sizeof_ragged_step()} vs {C.sizeof(SeistRaggedStep)}")
     _lib = L
     return L
 
@@ -255,6 +289,8 @@ EXPORTS = [
     "seist_sizeof_stream_step", "seist_stream_window", "seist_stream_stack", "seist_stream_emit", "seist_stream_keep",
     "seist_stream_history",
     "seist_stream_peaks_work_bytes", "seist_stream_peaks", "seist_stream_peaks_fill", "seist_stream_runs", "seist_stream_runs_fill",
+    "seist_sizeof_ragged_step", "seist_ragged_window", "seist_ragged_stack", "seist_ragged_emit", "seist_ragged_keep", "seist_ragged_ext",
+    "seist_ragged_peaks", "seist_ragged_peaks_fill", "seist_ragged_runs", "seist_ragged_runs_fill",
 ]
 
 

@@ -627,6 +627,303 @@ __global__ void __launch_bounds__(ST_NT) srun_fill_kernel(const float* __restric
   }
 }
 
+// ---- ragged streams: stations that advance at different rates (DESIGN §4.19) ----------------------------------------
+// One SeistRaggedStep per call; the per-station counts are device arrays, the call's data packed by the prefix arrays.
+
+// the last row r in [0, n) with off[r] <= j: the row whose packed range holds j (empty rows before it share its start);
+// always in [0, n), so malformed offsets pick a wrong row but never an out-of-range one
+__device__ __forceinline__ int rg_find(const int64_t* __restrict__ off, int n, long long j) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (off[mid] <= j) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// raw sample g of (s, c): the station's chunk block [r0, r1), the kept tail [r0 - min(W, r0), r0) before; 0.0f outside
+__device__ __forceinline__ float rg_raw(const SeistRaggedStep& p, const float* tail, const float* chunk, int s, int c, long long r0,
+                                        long long r1, long long g) {
+  if (g >= r0)
+    return g < r1 ? chunk[(size_t)p.C * p.chunk_off[s] + (size_t)c * (r1 - r0) + (size_t)(g - r0)] : 0.f;
+  const long long h = g - (r0 - min((long long)p.W, r0));
+  return h >= 0 ? tail[((size_t)s * p.C + c) * p.W + (size_t)h] : 0.f;
+}
+
+// x (B, C, W): row (b, c) = normalised window j0 + b of the call; zero from n_win on
+__global__ void __launch_bounds__(PR_NT) ragged_window_kernel(SeistRaggedStep p, const float* __restrict__ tail,
+                                                              const float* __restrict__ chunk, long long j0, float* __restrict__ x) {
+  extern __shared__ float rw_row[];                 // [W]
+  const int b = blockIdx.x / p.C, c = blockIdx.x % p.C;
+  const long long j = j0 + b;
+  float* dst = x + (size_t)blockIdx.x * p.W;
+  if (j >= p.n_win) {
+    for (int i = threadIdx.x; i < p.W; i += PR_NT) dst[i] = 0.f;
+    return;
+  }
+  const int s = rg_find(p.win_off, p.S, j);
+  const long long q = j - p.win_off[s], r0 = p.r0[s], r1 = p.r1[s];
+  const long long a = q < p.nk[s] ? (p.k0[s] + q) * p.P : p.tail[s];
+  for (int i = threadIdx.x; i < p.W; i += PR_NT) rw_row[i] = rg_raw(p, tail, chunk, s, c, r0, r1, a + i);
+  __syncthreads();
+  pr_normalize_row(rw_row, dst, p.W, p.norm_mode);
+}
+
+// stream_stack_kernel per station: CTA (x, s - s0, c) gathers the batch's windows of station s into its acc block
+__global__ void __launch_bounds__(ST_NT) ragged_stack_kernel(SeistRaggedStep p, const float* __restrict__ y, long long j0, int nb, int s0,
+                                                             const float* __restrict__ carry, float* __restrict__ acc) {
+  const int s = s0 + blockIdx.y, c = blockIdx.z;
+  if (s >= p.S) return;
+  const long long wb = p.win_off[s], nw = p.win_off[s + 1] - wb;
+  const long long qa = max(j0 - wb, 0LL), qb = min(j0 + nb - 1 - wb, nw - 1);
+  if (qa > qb) return;
+  const long long nk = p.nk[s], k0 = p.k0[s], tl0 = p.tail[s], f0 = p.f0[s], r1 = p.r1[s];
+  const long long sa = qa < nk ? (k0 + qa) * p.P : tl0, sb = qb < nk ? (k0 + qb) * p.P : tl0;
+  const long long t = sa + blockIdx.x * (long long)ST_NT + threadIdx.x;
+  if (t >= sb + p.W || t < f0 || t >= r1) return;
+  const long long lo = t < p.W ? 0 : (t - p.W) / p.P + 1, hi = min(t / p.P, k0 + nk - 1);
+  const bool reg = lo <= hi;                                   // else the tail window is t's only one
+  const bool tl = tl0 >= 0 && qb == nw - 1 && t >= tl0;
+  const bool first = reg ? (qa < nk && lo >= k0 + qa) : tl;
+  const long long L = r1 - f0;
+  float* out = acc + (size_t)3 * p.acc_off[s] + (size_t)c * L + (size_t)(t - f0);
+  float a = first ? (p.stack_mode == 0 ? 0.f : -INFINITY)
+                  : (qa > 0 ? *out : (t - f0 < p.W ? carry[((size_t)s * 3 + c) * p.W + (size_t)(t - f0)] : 0.f));
+  const float* yb = y + (size_t)c * p.W;
+  const long long kb = min(hi, k0 + min(qb, nk - 1));
+  for (long long k = max(lo, k0 + qa); k <= kb; ++k) {
+    const float v = yb[(size_t)(wb + (k - k0) - j0) * 3 * p.W + (size_t)(t - k * p.P)];
+    a = p.stack_mode == 0 ? a + v : fmaxf(a, v);
+  }
+  if (tl) {
+    const float v = yb[(size_t)(wb + nk - j0) * 3 * p.W + (size_t)(t - tl0)];
+    a = p.stack_mode == 0 ? a + v : fmaxf(a, v);
+  }
+  *out = a;
+}
+
+// CTA (x, s, c): probs block of s = final [f0, f1), carry_out = partial sums of [f1, r1), as stream_emit_kernel
+__global__ void __launch_bounds__(ST_NT) ragged_emit_kernel(SeistRaggedStep p, const float* __restrict__ carry, const float* __restrict__ acc,
+                                                            float* __restrict__ probs, float* __restrict__ carry_out) {
+  const int s = blockIdx.y, c = blockIdx.z;
+  const long long f0 = p.f0[s], r1 = p.r1[s], i = blockIdx.x * (long long)ST_NT + threadIdx.x;
+  if (i >= r1 - f0) return;
+  const long long t = f0 + i, f1 = p.f1[s], nk = p.nk[s], k0 = p.k0[s], tl0 = p.tail[s], kr = p.kr[s];
+  const bool touched = (nk > 0 && t >= k0 * p.P && t < (k0 + nk - 1) * p.P + p.W) || (tl0 >= 0 && t >= tl0);
+  const size_t row = (size_t)s * 3 + c;
+  float v = touched ? acc[(size_t)3 * p.acc_off[s] + (size_t)c * (r1 - f0) + (size_t)i]
+                    : (t < p.r0[s] && i < p.W ? carry[row * p.W + (size_t)i] : 0.f);   // t >= r0 untouched: no window yet
+  if (t < f1) {
+    if (p.stack_mode == 0) {
+      const long long lo = t < p.W ? 0 : (t - p.W) / p.P + 1, hi = kr >= 0 ? min(t / p.P, kr - 1) : t / p.P;
+      const int cnt = (int)max(hi - lo + 1, 0LL) + (tl0 >= 0 && t >= tl0 ? 1 : 0);
+      v = __fdiv_rn(v, (float)cnt);
+    }
+    probs[(size_t)3 * p.out_off[s] + (size_t)c * (f1 - f0) + (size_t)i] = v;
+  } else if (t - f1 < p.W) {
+    carry_out[row * p.W + (size_t)(t - f1)] = v;
+  }
+}
+
+// tail_out (S, C, W): the last min(W, r1[s]) raw samples of each station after the call
+__global__ void __launch_bounds__(ST_NT) ragged_keep_kernel(SeistRaggedStep p, const float* __restrict__ tail,
+                                                            const float* __restrict__ chunk, float* __restrict__ tail_out) {
+  const int s = blockIdx.y / p.C, c = blockIdx.y % p.C;
+  const long long r0 = p.r0[s], r1 = p.r1[s], keep = min((long long)p.W, r1);
+  const int i = blockIdx.x * ST_NT + threadIdx.x;
+  if (i < keep) tail_out[(size_t)blockIdx.y * p.W + i] = rg_raw(p, tail, chunk, s, c, r0, r1, r1 - keep + i);
+}
+
+// channel ch of row s of a packed ext, and its length
+__device__ __forceinline__ const float* rg_row(const float* ext, const long long* __restrict__ ext_off, int C, int ch, int s, long long& L) {
+  const long long e0 = ext_off[s];
+  L = ext_off[s + 1] - e0;
+  return ext + (size_t)C * e0 + (size_t)ch * L;
+}
+
+// CTA (x, s, c): ext row = look, the stretch, -inf; look_out = its samples m, m + 1
+__global__ void __launch_bounds__(ST_NT) ragged_ext_kernel(const float* __restrict__ look, const float* __restrict__ probs,
+                                                           const long long* __restrict__ prob_off, const long long* __restrict__ ext_off,
+                                                           int C, float* __restrict__ ext, float* __restrict__ look_out) {
+  const int s = blockIdx.y, c = blockIdx.z;
+  const long long e0 = ext_off[s], L = ext_off[s + 1] - e0, p0 = prob_off[s], m = prob_off[s + 1] - p0;
+  const long long i = blockIdx.x * (long long)ST_NT + threadIdx.x;
+  if (i >= L) return;
+  const float v = i < 2 ? look[((size_t)s * C + c) * 2 + i] : (i - 2 < m ? probs[(size_t)C * p0 + (size_t)c * m + (size_t)(i - 2)] : -INFINITY);
+  ext[(size_t)C * e0 + (size_t)c * L + (size_t)i] = v;
+  if (i == m || i == m + 1) look_out[((size_t)s * C + c) * 2 + (size_t)(i - m)] = v;
+}
+
+// pend_move_kernel with a rebase per row
+__global__ void __launch_bounds__(ST_NT) rg_pend_move_kernel(const int* __restrict__ pci, const float* __restrict__ pcv, int pcapc,
+                                                             const int* __restrict__ pnclosed, const int* __restrict__ pncand,
+                                                             const long long* __restrict__ delta, int* __restrict__ cidx,
+                                                             float* __restrict__ cval, int capc, int* __restrict__ npend) {
+  const int s = blockIdx.y;
+  const int a = pci ? pnclosed[s] : 0, m = pci ? pncand[s] - a : 0;
+  if (blockIdx.x == 0 && threadIdx.x == 0) npend[s] = m;
+  if (m == 0) return;
+  const long long d = delta[s];
+  for (int j = blockIdx.x * ST_NT + threadIdx.x; j < m; j += gridDim.x * ST_NT) {
+    cidx[(size_t)s * capc + j] = (int)(pci[(size_t)s * pcapc + a + j] - d);
+    cval[(size_t)s * capc + j] = pcv[(size_t)s * pcapc + a + j];
+  }
+}
+
+// the tested range of a row: [max(lo, 1), min(hi, L - 2)]
+__device__ __forceinline__ void rg_range(const long long* lo_a, const long long* hi_a, int s, long long L, long long lim_hi, long long& lo,
+                                         long long& hi) {
+  lo = max(lo_a[s], 1LL);
+  hi = min(hi_a[s], L - lim_hi);
+}
+
+// cand_count_kernel over each row's own range; blocks past it count 0
+__global__ void __launch_bounds__(ST_NT) rg_cand_count_kernel(const float* __restrict__ ext, const long long* __restrict__ ext_off, int C,
+                                                              int ch, const long long* __restrict__ lo_a, const long long* __restrict__ hi_a,
+                                                              float mph, int* __restrict__ blk, int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  long long L, lo, hi;
+  const float* x = rg_row(ext, ext_off, C, ch, blockIdx.y, L);
+  rg_range(lo_a, hi_a, blockIdx.y, L, 2, lo, hi);
+  const long long a = lo + (long long)blockIdx.x * ST_CH;
+  int n = 0;
+  for (long long i = a + threadIdx.x; i < min(a + ST_CH, hi + 1); i += ST_NT) n += pk_cand(x, (int)i, mph);
+  n = st_block_count(n, warp_s);
+  if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
+}
+
+// cand_fill_kernel with a per-row index shift, behind the row's pending candidates
+__global__ void __launch_bounds__(ST_NT) rg_cand_fill_kernel(const float* __restrict__ ext, const long long* __restrict__ ext_off, int C,
+                                                             int ch, const long long* __restrict__ lo_a, const long long* __restrict__ hi_a,
+                                                             float mph, const int* __restrict__ blk, int nblk, const int* __restrict__ off0,
+                                                             const long long* __restrict__ ishift, int capc, int* __restrict__ cidx,
+                                                             float* __restrict__ cval) {
+  __shared__ int warp_s[ST_NT / 32];
+  const int s = blockIdx.y;
+  long long L, lo, hi;
+  const float* x = rg_row(ext, ext_off, C, ch, s, L);
+  rg_range(lo_a, hi_a, s, L, 2, lo, hi);
+  const long long a = lo + (long long)blockIdx.x * ST_CH;
+  if (a > hi) return;                                          // the whole CTA: past the row's range
+  const int sh = (int)ishift[s];
+  int base = blk[(size_t)s * nblk + blockIdx.x] + off0[s];
+  int* ci = cidx + (size_t)s * capc;
+  float* cv = cval + (size_t)s * capc;
+  for (long long i0 = a; i0 < min(a + ST_CH, hi + 1); i0 += ST_NT) {
+    const long long i = i0 + threadIdx.x;
+    const bool f = i <= hi && pk_cand(x, (int)i, mph);
+    int tot;
+    const int r = st_block_rank(f, warp_s, tot);
+    if (f && base + r < capc) { ci[base + r] = (int)i + sh; cv[base + r] = x[i]; }
+    base += tot;
+  }
+}
+
+// close_scan_kernel with lim and base per row
+__global__ void __launch_bounds__(ST_NT) rg_close_scan_kernel(const int* __restrict__ npend, const int* __restrict__ nnew,
+                                                              const int* __restrict__ cidx, int capc, int mpd,
+                                                              const long long* __restrict__ lim_a, const long long* __restrict__ base_a,
+                                                              int* __restrict__ ncand, int* __restrict__ nclosed, long long* __restrict__ info) {
+  __shared__ int last_s;
+  const int s = blockIdx.x, n = min(npend[s] + nnew[s], capc);
+  const int* ci = cidx + (size_t)s * capc;
+  if (threadIdx.x == 0) last_s = 0;
+  __syncthreads();
+  for (int top = n - 1; top >= 1; top -= ST_NT) {            // the last cluster start, searched from the end
+    const int j = top - (int)threadIdx.x;
+    const bool f = j >= 1 && ci[j] - ci[j - 1] > mpd;
+    if (f) atomicMax(&last_s, j);
+    if (__syncthreads_or(f)) break;
+  }
+  if (threadIdx.x == 0) {
+    const int nc = n == 0 || (long long)ci[n - 1] + mpd <= lim_a[s] ? n : last_s;
+    ncand[s] = n;
+    nclosed[s] = nc;
+    info[s] = n - nc;
+    info[gridDim.x + s] = nc < n ? base_a[s] + ci[nc] : LLONG_MAX;
+  }
+}
+
+// keep_fill_kernel with the index base per row
+__global__ void __launch_bounds__(ST_NT) rg_keep_fill_kernel(const int* __restrict__ ncand, int capc, const int* __restrict__ cidx,
+                                                             const float* __restrict__ cval, const unsigned char* __restrict__ state,
+                                                             const int* __restrict__ blk, int nblk, const long long* __restrict__ offsets,
+                                                             const long long* __restrict__ base_a, long long* __restrict__ index,
+                                                             float* __restrict__ value) {
+  __shared__ int warp_s[ST_NT / 32];
+  const int n = ncand[blockIdx.y];
+  const int a = blockIdx.x * ST_CH;
+  if (a >= n) return;
+  const size_t r0 = (size_t)blockIdx.y * capc;
+  const long long sh = base_a[blockIdx.y];
+  long long b = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  for (int j0 = a; j0 < min(a + ST_CH, n); j0 += ST_NT) {
+    const int j = j0 + threadIdx.x;
+    const bool f = j < n && state[r0 + j] == CL_KEEP;
+    int tot;
+    const int r = st_block_rank(f, warp_s, tot);
+    if (f) { index[b + r] = cidx[r0 + j] + sh; value[b + r] = cval[r0 + j]; }
+    b += tot;
+  }
+}
+
+// srun_count_kernel over each row's own range [max(lo, 1), min(hi, L - 1)]
+__global__ void __launch_bounds__(ST_NT) rg_srun_count_kernel(const float* __restrict__ ext, const long long* __restrict__ ext_off, int C,
+                                                              int ch, const long long* __restrict__ lo_a, const long long* __restrict__ hi_a,
+                                                              float thr, int* __restrict__ blk, int nblk, const long long* __restrict__ open_in,
+                                                              long long* __restrict__ open_out) {
+  __shared__ int warp_s[ST_NT / 32];
+  long long L, lo, hi;
+  const float* x = rg_row(ext, ext_off, C, ch, blockIdx.y, L);
+  rg_range(lo_a, hi_a, blockIdx.y, L, 1, lo, hi);
+  hi = max(hi, lo - 1);
+  const long long a = lo + (long long)blockIdx.x * ST_CH;
+  int n = 0;
+  for (long long i = a + threadIdx.x; i < min(a + ST_CH, hi + 1); i += ST_NT) n += sr_off(x, (int)i, thr);
+  n = st_block_count(n, warp_s);
+  if (threadIdx.x == 0) {
+    blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
+    if (blockIdx.x == 0) open_out[blockIdx.y] = x[hi] > thr ? open_in[blockIdx.y] : -1;   // raised by the fill on a new start
+  }
+}
+
+// srun_fill_kernel with lo, hi and g0 per row
+__global__ void __launch_bounds__(ST_NT) rg_srun_fill_kernel(const float* __restrict__ ext, const long long* __restrict__ ext_off, int C,
+                                                             int ch, const long long* __restrict__ lo_a, const long long* __restrict__ hi_a,
+                                                             float thr, const long long* __restrict__ g0_a, const int* __restrict__ blk,
+                                                             int nblk, const long long* __restrict__ offsets,
+                                                             const long long* __restrict__ open_in, long long* __restrict__ open_out,
+                                                             long long* __restrict__ pairs) {
+  __shared__ int warp_s[ST_NT / 32];
+  const int s = blockIdx.y;
+  long long L, lo, hi;
+  const float* x = rg_row(ext, ext_off, C, ch, s, L);
+  rg_range(lo_a, hi_a, s, L, 1, lo, hi);
+  hi = max(hi, lo - 1);
+  const long long end = offsets[s + 1];
+  if (blockIdx.x == 0 && threadIdx.x == 0 && open_in[s] >= 0 && end > offsets[s]) pairs[offsets[s] * 2] = open_in[s];
+  const long long a = lo + (long long)blockIdx.x * ST_CH;
+  if (a > hi) return;                                          // the whole CTA: past the row's range
+  const long long g0 = g0_a[s];
+  const bool open_end = x[hi] > thr;
+  long long off_base = offsets[s] + blk[(size_t)s * nblk + blockIdx.x];
+  long long on_base = off_base + (x[a - 1] > thr ? 1 : 0);    // a run open into the block ends before the next starts
+  for (long long i0 = a; i0 < min(a + ST_CH, hi + 1); i0 += ST_NT) {
+    const long long i = i0 + threadIdx.x;
+    const bool fon = i <= hi && sr_on(x, (int)i, thr), foff = i <= hi && sr_off(x, (int)i, thr);
+    int ton, toff;
+    const int ron = st_block_rank(fon, warp_s, ton);
+    const int roff = st_block_rank(foff, warp_s, toff);
+    if (foff) pairs[(off_base + roff) * 2 + 1] = g0 + i - 1;
+    if (fon) {
+      if (on_base + ron < end) pairs[(on_base + ron) * 2] = g0 + i;
+      else if (open_end) atomicMax(&open_out[s], g0 + i);
+    }
+    on_base += ton;
+    off_base += toff;
+  }
+}
+
 // ---- work buffers ---------------------------------------------------------------------------------------------------
 __host__ __device__ inline size_t st_align(size_t b) { return (b + 255) & ~(size_t)255; }
 inline int st_capc(int T) { return T / 2 + 1; }                 // candidates of a row: never two adjacent samples
@@ -1015,6 +1312,182 @@ int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t chann
                                                                     (long long*)open_out, (long long*)pairs);
   note_launch();
   return check_launch("stream_runs_fill");
+}
+
+uint64_t seist_sizeof_ragged_step(void) { return sizeof(SeistRaggedStep); }
+
+static bool rg_ok(const SeistRaggedStep* p) {
+  return p && p->f0 && p->r0 && p->f1 && p->r1 && p->k0 && p->nk && p->tail && p->kr && p->win_off && p->chunk_off && p->acc_off &&
+         p->out_off && p->S > 0 && p->S <= 65535 && p->C > 0 && p->W >= 1 && p->W <= 49152 && p->P >= 1 && p->P <= p->W &&
+         p->n_win >= 0 && p->max_len >= 0 && p->max_len <= INT32_MAX && p->norm_mode >= 0 && p->norm_mode <= 2 &&
+         p->stack_mode >= 0 && p->stack_mode <= 1;
+}
+
+int seist_ragged_window(const SeistRaggedStep* step, const float* tail_raw, const float* chunk, int64_t j0, int32_t B, float* x,
+                        void* stream) {
+  if (!rg_ok(step) || !tail_raw || !chunk || !x || j0 < 0 || B <= 0 || (long long)B * step->C > INT32_MAX) {
+    set_error("ragged_window: bad arguments (a consistent SeistRaggedStep, W <= 49152, non-null tail_raw and chunk, j0 >= 0, B > 0)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * step->W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(ragged_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  ragged_window_kernel<<<(unsigned)((long long)B * step->C), PR_NT, smem, (cudaStream_t)stream>>>(*step, tail_raw, chunk, j0, x);
+  note_launch();
+  return check_launch("ragged_window");
+}
+
+int seist_ragged_stack(const SeistRaggedStep* step, const float* y, int64_t j0, int32_t B, int32_t s0, int32_t s1,
+                       const float* carry, float* acc, void* stream) {
+  if (!rg_ok(step) || !y || !carry || !acc || j0 < 0 || B <= 0 || s0 < 0 || s1 < s0 || s1 >= step->S) {
+    set_error("ragged_stack: bad arguments (a consistent SeistRaggedStep, j0 >= 0, B > 0, 0 <= s0 <= s1 < S)");
+    return -1;
+  }
+  const SeistRaggedStep& p = *step;
+  if (j0 >= p.n_win) return 0;
+  const int nb = (int)std::min<long long>(B, p.n_win - j0);
+  const long long span = std::min<long long>(p.max_len, (long long)(nb - 1) * p.P + p.W);
+  if (span == 0) return 0;
+  const dim3 grid((unsigned)((span + ST_NT - 1) / ST_NT), (unsigned)(s1 - s0 + 1), 3);
+  ragged_stack_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(p, y, j0, nb, s0, carry, acc);
+  note_launch();
+  return check_launch("ragged_stack");
+}
+
+int seist_ragged_emit(const SeistRaggedStep* step, const float* carry, const float* acc, float* probs, float* carry_out,
+                      void* stream) {
+  if (!rg_ok(step) || !carry || !acc || !probs || !carry_out || carry_out == carry) {
+    set_error("ragged_emit: bad arguments (a consistent SeistRaggedStep, non-null buffers, carry_out distinct from carry)");
+    return -1;
+  }
+  if (step->max_len == 0) return 0;
+  const dim3 grid((unsigned)((step->max_len + ST_NT - 1) / ST_NT), (unsigned)step->S, 3);
+  ragged_emit_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(*step, carry, acc, probs, carry_out);
+  note_launch();
+  return check_launch("ragged_emit");
+}
+
+int seist_ragged_keep(const SeistRaggedStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream) {
+  if (!rg_ok(step) || !tail_raw || !chunk || !tail_out || tail_out == tail_raw || step->S * step->C > 65535) {
+    set_error("ragged_keep: bad arguments (a consistent SeistRaggedStep, S * C <= 65535, tail_out distinct from tail_raw)");
+    return -1;
+  }
+  const dim3 grid((unsigned)((step->W + ST_NT - 1) / ST_NT), (unsigned)(step->S * step->C));
+  ragged_keep_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(*step, tail_raw, chunk, tail_out);
+  note_launch();
+  return check_launch("ragged_keep");
+}
+
+int seist_ragged_ext(const float* look, const float* probs, const int64_t* prob_off, const int64_t* ext_off, int32_t S, int32_t C,
+                     int64_t max_L, float* ext, float* look_out, void* stream) {
+  if (!look || !probs || !prob_off || !ext_off || !ext || !look_out || look_out == look || S <= 0 || S > 65535 || C <= 0 ||
+      C > 65535 || max_L < 2 || max_L > INT32_MAX) {
+    set_error("ragged_ext: bad arguments (non-null buffers, look_out distinct from look, S, C <= 65535, 2 <= max_L < 2^31)");
+    return -1;
+  }
+  const dim3 grid((unsigned)((max_L + ST_NT - 1) / ST_NT), (unsigned)S, (unsigned)C);
+  ragged_ext_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(look, probs, (const long long*)prob_off, (const long long*)ext_off, C, ext,
+                                                              look_out);
+  note_launch();
+  return check_launch("ragged_ext");
+}
+
+static bool rg_rows_ok(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L, const int64_t* lo,
+                       const int64_t* hi, int64_t max_span) {
+  return ext && ext_off && lo && hi && S > 0 && S <= 65535 && channel >= 0 && channel < C && max_L >= 2 && max_L <= INT32_MAX &&
+         max_span >= 0 && max_span <= max_L;
+}
+
+int seist_ragged_peaks(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
+                       const int64_t* lo, const int64_t* hi, int64_t max_span, float mph, int32_t min_peak_dist,
+                       const int64_t* lim, const int64_t* base, const int64_t* ishift, void* work, int32_t capc,
+                       const void* prev, int32_t prev_capc, int64_t prev_L, const int64_t* delta, int32_t max_pend,
+                       int64_t* counts, int64_t* info, void* stream) {
+  if (!rg_rows_ok(ext, ext_off, S, C, channel, max_L, lo, hi, max_span) || !lim || !base || !ishift || !work || !counts || !info ||
+      min_peak_dist <= 1 || max_pend < 0 || (long long)capc < (long long)max_pend + max_L / 2 + 1 ||
+      (prev && (!delta || prev_capc < 1 || prev_L < 2 || prev_L > INT32_MAX))) {
+    set_error("ragged_peaks: bad arguments (2 <= max_L < 2^31, 0 <= max_span <= max_L, S <= 65535, min_peak_dist > 1, "
+              "capc >= max_pend + max_L / 2 + 1, per-row arrays non-null)");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const StreamPeakWork w(work, S, capc, max_L);
+  const int nb = std::max(1, st_nblk((int)max_span)), nbc = st_nblk(capc);
+  const StreamPeakWork pw(prev, S, prev ? prev_capc : 1, prev ? prev_L : 2);
+  const long long* eo = (const long long*)ext_off;
+  const long long *lo_a = (const long long*)lo, *hi_a = (const long long*)hi;
+  rg_pend_move_kernel<<<dim3(std::max(1, (max_pend + ST_NT - 1) / ST_NT), S), ST_NT, 0, st>>>(
+      prev ? pw.cidx : nullptr, pw.cval, prev_capc, pw.nclosed, pw.ncand, (const long long*)delta, w.cidx, w.cval, capc, w.npend);
+  rg_cand_count_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(ext, eo, C, channel, lo_a, hi_a, mph, w.blk, nb);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nb, w.nnew, nullptr);
+  rg_cand_fill_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(ext, eo, C, channel, lo_a, hi_a, mph, w.blk, nb, w.npend,
+                                                     (const long long*)ishift, capc, w.cidx, w.cval);
+  rg_close_scan_kernel<<<S, ST_NT, 0, st>>>(w.npend, w.nnew, w.cidx, capc, min_peak_dist, (const long long*)lim, (const long long*)base,
+                                            w.ncand, w.nclosed, (long long*)info);
+  cluster_kernel<<<dim3((capc + CL_SEG - 1) / CL_SEG, S), ST_NT, 0, st>>>(w.nclosed, capc, w.cidx, w.cval, w.state, min_peak_dist);
+  keep_count_kernel<<<dim3(nbc, S), ST_NT, 0, st>>>(w.nclosed, capc, w.state, w.blk, nbc);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nbc, w.nkeep, (long long*)counts);
+  for (int i = 0; i < 8; ++i) note_launch();
+  return check_launch("ragged_peaks");
+}
+
+int seist_ragged_peaks_fill(int32_t S, int64_t max_L, const void* work, int32_t capc, const int64_t* base, const int64_t* offsets,
+                            int64_t* index, float* value, void* stream) {
+  if (!work || !base || !offsets || !index || !value || S <= 0 || S > 65535 || max_L < 2 || max_L > INT32_MAX || capc < 1) {
+    set_error("ragged_peaks_fill: bad arguments (the work buffer of the seist_ragged_peaks call, non-null outputs)");
+    return -1;
+  }
+  const StreamPeakWork w(const_cast<void*>(work), S, capc, max_L);
+  const int nbc = st_nblk(capc);
+  rg_keep_fill_kernel<<<dim3(nbc, S), ST_NT, 0, (cudaStream_t)stream>>>(w.nclosed, capc, w.cidx, w.cval, w.state, w.blk, nbc,
+                                                                        (const long long*)offsets, (const long long*)base,
+                                                                        (long long*)index, value);
+  note_launch();
+  return check_launch("ragged_peaks_fill");
+}
+
+int seist_ragged_runs(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
+                      const int64_t* lo, const int64_t* hi, int64_t max_span, float threshold, const int64_t* open_in,
+                      int64_t* open_out, void* work, int64_t work_bytes, int64_t* counts, void* stream) {
+  if (!rg_rows_ok(ext, ext_off, S, C, channel, max_L, lo, hi, max_span) || !open_in || !open_out || !work || !counts ||
+      work_bytes < seist_runs_work_bytes(S, max_L)) {
+    set_error("ragged_runs: bad arguments (2 <= max_L < 2^31, 0 <= max_span <= max_L, S <= 65535, "
+              "work >= seist_runs_work_bytes(S, max_L))");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int* total = (int*)work;
+  int* blk = (int*)((char*)work + st_align(sizeof(int) * S));
+  const int nb = std::max(1, st_nblk((int)max_span));
+  rg_srun_count_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(ext, (const long long*)ext_off, C, channel, (const long long*)lo,
+                                                      (const long long*)hi, threshold, blk, nb, (const long long*)open_in,
+                                                      (long long*)open_out);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(blk, nb, total, (long long*)counts);
+  note_launch();
+  note_launch();
+  return check_launch("ragged_runs");
+}
+
+int seist_ragged_runs_fill(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
+                           const int64_t* lo, const int64_t* hi, int64_t max_span, float threshold, const int64_t* g0,
+                           const int64_t* open_in, int64_t* open_out, const void* work, int64_t work_bytes,
+                           const int64_t* offsets, int64_t* pairs, void* stream) {
+  if (!rg_rows_ok(ext, ext_off, S, C, channel, max_L, lo, hi, max_span) || !g0 || !open_in || !open_out || !work || !offsets ||
+      work_bytes < seist_runs_work_bytes(S, max_L)) {
+    set_error("ragged_runs_fill: bad arguments (the work buffer of the seist_ragged_runs call, per-row arrays non-null)");
+    return -1;
+  }
+  const int* blk = (const int*)((const char*)work + st_align(sizeof(int) * S));
+  const int nb = std::max(1, st_nblk((int)max_span));
+  rg_srun_fill_kernel<<<dim3(nb, S), ST_NT, 0, (cudaStream_t)stream>>>(ext, (const long long*)ext_off, C, channel, (const long long*)lo,
+                                                                       (const long long*)hi, threshold, (const long long*)g0, blk, nb,
+                                                                       (const long long*)offsets, (const long long*)open_in,
+                                                                       (long long*)open_out, (long long*)pairs);
+  note_launch();
+  return check_launch("ragged_runs_fill");
 }
 
 }  // extern "C"

@@ -15,6 +15,7 @@ from __future__ import annotations
 
 from typing import List, NamedTuple, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -398,6 +399,384 @@ class ContinuousStream:
         return StreamOutput(t0, probs, ppk, spk, det)
 
 
+# ---- ragged streams: stations that advance at different rates (DESIGN §4.19) -----------------------------------------
+_RG_COUNTS = ("f0", "r0", "f1", "r1", "k0", "nk", "tail", "kr")
+_RG_OFFS = ("win_off", "chunk_off", "acc_off", "out_off")
+
+
+def _prefix(counts) -> np.ndarray:
+    return np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)
+
+
+def ragged_plan(R, n, window: int, stride: int, close: bool = False) -> dict:
+    """The per-station counts of one call of a ragged stream, from the samples pushed so far R (S,) and this push's
+    lengths n (S,) (ignored at the close), by the §4.16 finality rules applied to each station: f0 = max(0, R - W) samples
+    are final before the call, k0 = the next regular window; a push runs the regular windows that end by R + n and makes
+    max(0, R + n - W) final; the close runs the station's tail window (start T - W, when the last regular window ends
+    before T = R) and makes T final.  Returns numpy int64 arrays f0, r0, f1, r1, k0, nk, tail, kr (S,) and the exclusive
+    prefix arrays win_off, chunk_off, acc_off, out_off (S + 1,).  Raises ValueError naming the stations with T < W at the
+    close."""
+    W, P = int(window), int(stride)
+    R = np.asarray(R, dtype=np.int64).reshape(-1)
+    f0 = np.maximum(R - W, 0)
+    k0 = np.where(R >= W, (R - W) // P + 1, 0)
+    if close:
+        short = np.nonzero(R < W)[0]
+        if short.size:
+            raise ValueError(f"stations {short.tolist()} hold fewer samples than one window ({W}): "
+                             f"{R[short].tolist()}")
+        kr = (R - W) // P + 1
+        tail = np.where((kr - 1) * P + W < R, R - W, -1)
+        r1, f1, nk = R.copy(), R.copy(), np.zeros_like(R)
+    else:
+        n = np.asarray(n, dtype=np.int64).reshape(-1)
+        if n.shape != R.shape or (n < 0).any():
+            raise ValueError(f"expected {R.size} non-negative lengths, got {n.tolist()}")
+        r1 = R + n
+        f1 = np.maximum(r1 - W, 0)
+        nk = np.where(r1 >= W, (r1 - W) // P + 1, 0) - k0
+        tail = np.full_like(R, -1)
+        kr = np.full_like(R, -1)
+    plan = dict(f0=f0, r0=R.copy(), f1=f1, r1=r1, k0=k0, nk=nk, tail=tail, kr=kr)
+    plan["win_off"] = _prefix(nk + (tail >= 0))
+    plan["chunk_off"] = _prefix(r1 - R)
+    plan["acc_off"] = _prefix(r1 - f0)
+    plan["out_off"] = _prefix(f1 - f0)
+    return plan
+
+
+def ragged_window_ids(plan: dict, stride: int) -> list:
+    """The call's packed windows in order as (station, start): each station's regular windows, then its tail window."""
+    ids = []
+    for s in range(len(plan["f0"])):
+        ids += [(s, (int(plan["k0"][s]) + q) * int(stride)) for q in range(int(plan["nk"][s]))]
+        if plan["tail"][s] >= 0:
+            ids.append((s, int(plan["tail"][s])))
+    return ids
+
+
+def _upload(host: np.ndarray, device) -> torch.Tensor:
+    """One small host-to-device copy from pinned memory that does not synchronise the host."""
+    return torch.from_numpy(np.ascontiguousarray(host, dtype=np.int64)).pin_memory().to(device, non_blocking=True)
+
+
+class RaggedStep:
+    """One call of a ragged stream: the host plan (`ragged_plan`), its device copy and the SeistRaggedStep pointing into it."""
+
+    def __init__(self, plan: dict, C: int, window: int, stride: int, norm_mode: str = "std", stack: str = "mean", device=None,
+                 dev: torch.Tensor | None = None):
+        self.plan = plan
+        self.S = S = len(plan["f0"])
+        self.host = np.concatenate([plan[k] for k in _RG_COUNTS + _RG_OFFS]).astype(np.int64)
+        self.dev = _upload(self.host, device) if dev is None else dev
+        if self.dev.dtype != torch.int64 or self.dev.numel() < self.host.size or not self.dev.is_cuda:
+            raise ValueError("the device copy of a ragged step must be an int64 CUDA tensor holding its plan")
+        ptr = [self.dev.data_ptr() + 8 * S * i for i in range(len(_RG_COUNTS))]
+        base = self.dev.data_ptr() + 8 * S * len(_RG_COUNTS)
+        ptr += [base + 8 * (S + 1) * i for i in range(len(_RG_OFFS))]
+        self.n_win = int(plan["win_off"][-1])
+        self.max_len = int((plan["r1"] - plan["f0"]).max(initial=0))
+        self.desc = _lib.SeistRaggedStep(*ptr, n_win=self.n_win, max_len=self.max_len, S=S, C=int(C), W=int(window), P=int(stride),
+                                         norm_mode=_MODES[norm_mode], stack_mode=_STACK[stack])
+
+    def stations(self, j0: int, B: int):
+        """The first and last station of windows j0 .. min(j0 + B, n_win) - 1."""
+        off = self.plan["win_off"]
+        j1 = min(j0 + B, self.n_win) - 1
+        return int(np.searchsorted(off, j0, "right") - 1), int(np.searchsorted(off, j1, "right") - 1)
+
+
+def ragged_stream_step(C: int, window: int, stride: int, R, n, close: bool = False, norm_mode: str = "std", stack: str = "mean",
+                       device="cuda") -> RaggedStep:
+    """The ragged counterpart of `stream_step`: one call of a ragged stream from the per-station counts R and lengths n."""
+    return RaggedStep(ragged_plan(R, n, window, stride, close), C, window, stride, norm_mode, stack, device)
+
+
+def _flat(t: torch.Tensor, n: int, what: str, device):
+    if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() >= max(1, n) and t.device == device):
+        raise ValueError(f"{what}: expected a contiguous float32 CUDA tensor on {device} of at least {max(1, n)} elements, "
+                         f"got {tuple(t.shape)} {t.dtype} on {t.device}")
+
+
+def ragged_window_(x: torch.Tensor, step: RaggedStep, tail_raw: torch.Tensor, chunk: torch.Tensor, j0: int) -> torch.Tensor:
+    """Fill x (B, C, W) with the normalised windows j0 .. j0 + B - 1 of the call, cut from tail_raw (S, C, W) followed by
+    each station's (C, n_s) block of the packed chunk; ids from n_win on give zero rows."""
+    d = step.desc
+    _dense(tail_raw, (d.S, d.C, d.W), "kept raw samples")
+    _dense(x, (None, d.C, d.W), "window batch", tail_raw.device)
+    _flat(chunk, d.C * int(step.plan["chunk_off"][-1]), "packed chunk", tail_raw.device)
+    _lib.check(_lib.lib().seist_ragged_window(_ref(d), tail_raw.data_ptr(), chunk.data_ptr(), j0, x.shape[0], x.data_ptr(), _s()),
+               "seist_ragged_window")
+    return x
+
+
+def ragged_stack_(acc: torch.Tensor, y: torch.Tensor, step: RaggedStep, j0: int, carry: torch.Tensor) -> torch.Tensor:
+    """Stack the (B, 3, W) outputs of the call's windows j0 .. j0 + B - 1 into the packed partial sums acc (station s a
+    (3, r1 - f0) block at 3 * acc_off[s]); carry (S, 3, W) holds the partial sums of [f0, r0).  Batches in order from 0."""
+    d = step.desc
+    _dense(carry, (d.S, 3, d.W), "carry")
+    _flat(acc, 3 * int(step.plan["acc_off"][-1]), "partial sums", carry.device)
+    _dense(y, (None, 3, d.W), "window outputs", carry.device)
+    if j0 >= step.n_win:
+        return acc
+    s0, s1 = step.stations(j0, y.shape[0])
+    _lib.check(_lib.lib().seist_ragged_stack(_ref(d), y.data_ptr(), j0, y.shape[0], s0, s1, carry.data_ptr(), acc.data_ptr(), _s()),
+               "seist_ragged_stack")
+    return acc
+
+
+def ragged_emit_(probs: torch.Tensor, carry_out: torch.Tensor, step: RaggedStep, carry: torch.Tensor, acc: torch.Tensor) -> torch.Tensor:
+    """probs (packed, station s a (3, f1 - f0) block at 3 * out_off[s]) = the final probabilities; carry_out (S, 3, W) =
+    the partial sums of [f1, r1)."""
+    d = step.desc
+    _dense(carry, (d.S, 3, d.W), "carry")
+    _dense(carry_out, (d.S, 3, d.W), "carry_out", carry.device)
+    _flat(acc, 3 * int(step.plan["acc_off"][-1]), "partial sums", carry.device)
+    _flat(probs, 3 * int(step.plan["out_off"][-1]), "probs", carry.device)
+    if carry_out.data_ptr() == carry.data_ptr():
+        raise ValueError("carry_out must not be carry")
+    _lib.check(_lib.lib().seist_ragged_emit(_ref(d), carry.data_ptr(), acc.data_ptr(), probs.data_ptr(), carry_out.data_ptr(), _s()),
+               "seist_ragged_emit")
+    return probs
+
+
+def ragged_keep_(tail_out: torch.Tensor, step: RaggedStep, tail_raw: torch.Tensor, chunk: torch.Tensor) -> torch.Tensor:
+    """tail_out (S, C, W) = the last min(W, r1[s]) raw samples of each station after the call."""
+    d = step.desc
+    _dense(tail_raw, (d.S, d.C, d.W), "kept raw samples")
+    _dense(tail_out, (d.S, d.C, d.W), "tail_out", tail_raw.device)
+    _flat(chunk, d.C * int(step.plan["chunk_off"][-1]), "packed chunk", tail_raw.device)
+    if tail_out.data_ptr() == tail_raw.data_ptr():
+        raise ValueError("tail_out must not be tail_raw")
+    _lib.check(_lib.lib().seist_ragged_keep(_ref(d), tail_raw.data_ptr(), chunk.data_ptr(), tail_out.data_ptr(), _s()),
+               "seist_ragged_keep")
+    return tail_out
+
+
+class RaggedStreamOutput(NamedTuple):
+    """What one call of a ragged stream made final: per station s, probs[s] (3, m_s) of samples [t0[s], t0[s] + m_s)
+    (views into one buffer); the picks and detection runs that closed, as StreamOutput's CSR tuples."""
+    t0: list
+    probs: list
+    ppk: tuple
+    spk: tuple
+    det: tuple
+
+
+class RaggedPickStream:
+    """PickStream whose rows take stretches of different lengths: `push(stretches)` takes S (3, m_s) float32 tensors, any
+    m_s >= 0; each row keeps its own final count F_s and is decided by the §4.16 rules on its own.  `t0` (an int or one
+    per row) is the global index of each row's first sample."""
+
+    def __init__(self, n_stations: int, device, min_peak_dist: int, ppk_threshold: float = 0.3, spk_threshold: float = 0.3,
+                 det_threshold: float = 0.5, t0=0):
+        if min_peak_dist is None or int(min_peak_dist) <= 1:
+            raise ValueError(f"min_peak_dist must be > 1 samples, got {min_peak_dist}")
+        if int(n_stations) < 1:
+            raise ValueError(f"need at least one station, got {n_stations}")
+        self.S, self.device, self.mpd = int(n_stations), torch.device(device), int(min_peak_dist)
+        if self.device.type == "cuda" and self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.thr = (float(det_threshold), float(ppk_threshold), float(spk_threshold))
+        self.t0 = np.broadcast_to(np.asarray(t0, dtype=np.int64), (self.S,)).copy()
+        self.F = self.t0.copy()
+        self.closed = False
+        self.look = torch.full((self.S, 3, 2), float("-inf"), device=self.device)
+        self.open = torch.full((self.S,), -1, dtype=torch.int64, device=self.device)
+        self.pend = {1: None, 2: None}        # per pick channel: (work, capc, max_L, base (S,)) of the previous call
+        self.max_pend = {1: 0, 2: 0}
+        self.first_pend = {1: np.full(self.S, _I64_MAX, np.int64), 2: np.full(self.S, _I64_MAX, np.int64)}
+        self._none = torch.zeros(1, device=self.device)
+
+    def push(self, probs):
+        """The next final stretch of every row (a sequence of S (3, m_s) tensors) -> (ppk, spk, det) that closed."""
+        return self._stretches(probs, False)
+
+    def close(self, probs=None):
+        """The last stretches: every pending cluster and open run closes; each row's sample F_s - 1 ends its record."""
+        if probs is None:
+            probs = [torch.empty(3, 0, device=self.device) for _ in range(self.S)]
+        return self._stretches(probs, True)
+
+    def _stretches(self, probs, last: bool):
+        if self.closed:
+            raise RuntimeError("the stream is closed")
+        if len(probs) != self.S:
+            raise ValueError(f"expected {self.S} stretches, got {len(probs)}")
+        for p in probs:
+            if not p.is_cuda:
+                raise RuntimeError("RaggedPickStream has no CPU path: the probabilities must live on a CUDA device")
+            _dense(p, (3, None), "probabilities", self.device)
+        m = np.array([p.shape[1] for p in probs], dtype=np.int64)
+        host, meta = self._plan(m, last)
+        flat = torch.cat([p.reshape(-1) for p in probs]) if m.sum() else self._none
+        return self._run(flat, m, last, host, _upload(host, self.device), meta)
+
+    def _plan(self, m: np.ndarray, last: bool):
+        """The per-row descriptor of one call on the host (raises before any launch) and its host-side sizes."""
+        S = self.S
+        f0, f1 = self.F, self.F + m
+        if last and (f1 - self.t0 < 3).any():
+            short = np.nonzero(f1 - self.t0 < 3)[0]
+            raise ValueError(f"rows {short.tolist()} are too short to pick ({(f1 - self.t0)[short].tolist()} samples)")
+        L = m + 2 + int(last)
+        max_L = int(L.max())
+        if max_L > _I32_MAX:
+            raise ValueError(f"a stretch of {int(m.max())} samples is too long for one call")
+        g0 = f0 - 2
+        lo = np.maximum(1, 3 - (f0 - self.t0))
+        hi = m.copy()
+        rlo = np.full(S, 2, np.int64)
+        rhi = m + 1 + int(last)
+        parts = [_prefix(m), _prefix(L), lo, hi, rlo, rhi, g0]
+        meta = {"max_L": max_L, "f1": f1, "span": int(max(0, (hi - lo + 1).max())), "rspan": int((rhi - rlo + 1).max()), "ch": {}}
+        for ch in (1, 2):
+            base = np.minimum(g0, self.first_pend[ch])
+            if (f1 - base >= _I32_MAX - 2).any():
+                raise RuntimeError(f"a cluster of candidates spans more than 2^31 samples (channel {ch})")
+            lim = np.full(S, _I64_MAX >> 1, np.int64) if last else f1 - 2 - base
+            prev = self.pend[ch]
+            delta = base - prev[3] if prev else np.zeros(S, np.int64)
+            parts += [lim, base, g0 - base, delta]
+            meta["ch"][ch] = (base, self.max_pend[ch] + max_L // 2 + 1)
+        return np.concatenate(parts).astype(np.int64), meta
+
+    def _run(self, flat: torch.Tensor, m: np.ndarray, last: bool, host: np.ndarray, dev: torch.Tensor, meta: dict):
+        S, lib, d, max_L = self.S, _lib.lib(), self.device, meta["max_L"]
+        ptr = dev.data_ptr()
+        prob_off, ext_off = ptr, ptr + 8 * (S + 1)
+        lo, hi, rlo, rhi, g0 = (ptr + 8 * (2 * (S + 1) + S * i) for i in range(5))
+        chp = {ch: [ptr + 8 * (2 * (S + 1) + S * (5 + 4 * k + i)) for i in range(4)] for k, ch in enumerate((1, 2))}
+        n_ext = int(host[2 * (S + 1) - 1])
+        ext = torch.empty(max(1, 3 * n_ext), device=d)
+        look_out = torch.empty(S, 3, 2, device=d)
+        _lib.check(lib.seist_ragged_ext(self.look.data_ptr(), flat.data_ptr(), prob_off, ext_off, S, 3, max_L, ext.data_ptr(),
+                                        look_out.data_ptr(), _s()), "seist_ragged_ext")
+        staged = []
+        for ch in (1, 2):
+            lim, base, ishift, delta = chp[ch]
+            capc = meta["ch"][ch][1]
+            prev = self.pend[ch]
+            nbytes = lib.seist_stream_peaks_work_bytes(S, capc, max_L)
+            work = torch.empty(nbytes, dtype=torch.uint8, device=d)
+            counts = torch.empty(S, dtype=torch.int64, device=d)
+            info = torch.empty(2 * S, dtype=torch.int64, device=d)
+            _lib.check(lib.seist_ragged_peaks(ext.data_ptr(), ext_off, S, 3, ch, max_L, lo, hi, meta["span"], self.thr[ch], self.mpd, lim,
+                                              base, ishift, work.data_ptr(), capc, prev[0].data_ptr() if prev else None,
+                                              prev[1] if prev else 0, prev[2] if prev else 0, delta, self.max_pend[ch],
+                                              counts.data_ptr(), info.data_ptr(), _s()), "seist_ragged_peaks")
+            staged.append((work, capc, _offsets(counts), info))
+        rbytes = lib.seist_runs_work_bytes(S, max_L)
+        rwork = torch.empty(rbytes, dtype=torch.uint8, device=d)
+        rcounts = torch.empty(S, dtype=torch.int64, device=d)
+        open_out = torch.empty(S, dtype=torch.int64, device=d)
+        _lib.check(lib.seist_ragged_runs(ext.data_ptr(), ext_off, S, 3, 0, max_L, rlo, rhi, meta["rspan"], self.thr[0],
+                                         self.open.data_ptr(), open_out.data_ptr(), rwork.data_ptr(), rbytes, rcounts.data_ptr(), _s()),
+                   "seist_ragged_runs")
+        roff = _offsets(rcounts)
+        tot = torch.cat([staged[0][2][-1:], staged[1][2][-1:], roff[-1:], staged[0][3], staged[1][3]]).tolist()   # the one host sync
+        out = []
+        for i, (ch, (work, capc, off, info)) in enumerate(zip((1, 2), staged)):
+            n = tot[i]
+            index = torch.empty(n, dtype=torch.int64, device=d)
+            value = torch.empty(n, dtype=torch.float32, device=d)
+            if n:
+                _lib.check(lib.seist_ragged_peaks_fill(S, max_L, work.data_ptr(), capc, chp[ch][1], off.data_ptr(), index.data_ptr(),
+                                                       value.data_ptr(), _s()), "seist_ragged_peaks_fill")
+            out.append((index, value, off))
+            o = 3 + 2 * S * i
+            self.max_pend[ch] = max(tot[o:o + S])
+            self.first_pend[ch] = np.array(tot[o + S:o + 2 * S], dtype=np.int64)
+            self.pend[ch] = (work, capc, max_L, meta["ch"][ch][0])
+        pairs = torch.empty(tot[2], 2, dtype=torch.int64, device=d)
+        _lib.check(lib.seist_ragged_runs_fill(ext.data_ptr(), ext_off, S, 3, 0, max_L, rlo, rhi, meta["rspan"], self.thr[0], g0,
+                                              self.open.data_ptr(), open_out.data_ptr(), rwork.data_ptr(), rbytes, roff.data_ptr(),
+                                              pairs.data_ptr() if pairs.numel() else None, _s()), "seist_ragged_runs_fill")
+        self.open = open_out
+        self.look = look_out
+        self.F = meta["f1"]
+        self.closed = last
+        return out[0], out[1], (pairs, roff)
+
+
+class RaggedStream:
+    """A record whose stations advance at different rates (`ContinuousAnnotator.open_ragged_stream`).  `push(chunks)` takes
+    S float32 tensors (C, n_s) on the model's device, any n_s >= 0 (0: no new data from that station); `close()` ends every
+    station's record at its own length.  Each station follows the §4.16 finality rules on its own counts, with sample
+    indices counted from its own first sample; the windows of all stations in a call share the batched forward.  Each
+    call returns a RaggedStreamOutput; per station, concatenated, its probs equal `annotate` of that station's record and
+    its picks / runs `pick_phases` / `detect_events` of it (DESIGN §4.19)."""
+
+    def __init__(self, ann: "ContinuousAnnotator", n_stations: int):
+        if int(n_stations) < 1:
+            raise ValueError(f"need at least one station, got {n_stations}")
+        self.ann = ann
+        self.S, self.C = int(n_stations), ann.in_channels
+        self.device = next(ann.model.parameters()).device
+        W = ann.window
+        self.tail = [torch.zeros(self.S, self.C, W, device=self.device) for _ in range(2)]
+        self.carry = [torch.zeros(self.S, 3, W, device=self.device) for _ in range(2)]
+        self.R = np.zeros(self.S, np.int64)
+        self.forwards = 0
+        self.picker = RaggedPickStream(self.S, self.device, ann.min_peak_dist, ann.thresholds["ppk"], ann.thresholds["spk"],
+                                       ann.thresholds["det"])
+        self._none = torch.zeros(1, device=self.device)
+
+    @property
+    def closed(self) -> bool:
+        return self.picker.closed
+
+    @torch.no_grad()
+    def push(self, chunks) -> RaggedStreamOutput:
+        if self.closed:
+            raise RuntimeError("push() after close()")
+        if len(chunks) != self.S:
+            raise ValueError(f"expected {self.S} chunks (one per station), got {len(chunks)}")
+        for s, c in enumerate(chunks):
+            if not torch.is_tensor(c) or not c.is_cuda:
+                raise RuntimeError(f"station {s}: RaggedStream has no CPU path, the chunk must live on the model's CUDA device")
+            if c.device != self.device:
+                raise RuntimeError(f"station {s}: chunk on {c.device}, model on {self.device}")
+            if c.dtype != torch.float32 or c.dim() != 2 or c.shape[0] != self.C:
+                raise ValueError(f"station {s}: expected a ({self.C}, n) float32 chunk, got {tuple(c.shape)} {c.dtype}")
+            if not c.is_contiguous():
+                raise ValueError(f"station {s}: the chunk must be contiguous")
+        plan = ragged_plan(self.R, [c.shape[1] for c in chunks], self.ann.window, self.ann.stride)
+        chunk = torch.cat([c.reshape(-1) for c in chunks]) if plan["chunk_off"][-1] else self._none
+        return self._call(plan, chunk, False)
+
+    @torch.no_grad()
+    def close(self) -> RaggedStreamOutput:
+        if self.closed:
+            raise RuntimeError("close() after close()")
+        return self._call(ragged_plan(self.R, None, self.ann.window, self.ann.stride, close=True), self._none, True)
+
+    def _call(self, plan: dict, chunk: torch.Tensor, last: bool) -> RaggedStreamOutput:
+        ann, W = self.ann, self.ann.window
+        m = plan["f1"] - plan["f0"]
+        pick_host, meta = self.picker._plan(m, last)
+        nstep = len(_RG_COUNTS) * self.S + len(_RG_OFFS) * (self.S + 1)
+        host = np.concatenate([np.concatenate([plan[k] for k in _RG_COUNTS + _RG_OFFS]), pick_host])
+        dev = _upload(host, self.device)                             # the call's one descriptor copy
+        step = RaggedStep(plan, self.C, W, ann.stride, ann.norm_mode, ann.stack, self.device, dev[:nstep])
+        acc = torch.empty(max(1, 3 * int(plan["acc_off"][-1])), device=self.device)
+        for j0 in range(0, step.n_win, ann.batch):
+            ragged_window_(ann.graph.x, step, self.tail[0], chunk, j0)
+            y = ann.graph.replay()
+            ragged_stack_(acc, y, step, j0, self.carry[0])
+            self.forwards += 1
+        out = plan["out_off"]
+        probs = torch.empty(max(1, 3 * int(out[-1])), device=self.device)
+        ragged_emit_(probs, self.carry[1], step, self.carry[0], acc)
+        ragged_keep_(self.tail[1], step, self.tail[0], chunk)
+        self.tail.reverse()
+        self.carry.reverse()
+        self.R = plan["r1"].copy()
+        ppk, spk, det = self.picker._run(probs, m, last, pick_host, dev[nstep:], meta)
+        views = [probs[3 * int(out[s]):3 * int(out[s + 1])].view(3, int(m[s])) for s in range(self.S)]
+        return RaggedStreamOutput(plan["f0"].tolist(), views, ppk, spk, det)
+
+
 class ContinuousAnnotator:
     """`ann = ContinuousAnnotator(model, window=8192, stride=4096, batch=256, norm_mode="std", stack="mean")`
 
@@ -408,6 +787,8 @@ class ContinuousAnnotator:
     * `ann.detect_events(probs, det_threshold)` -> (pairs (E, 2), offsets (S + 1,)).
     * `st = ann.open_stream(n_stations)`: the same, chunk by chunk (`st.push(chunk)`, `st.close()`, ContinuousStream);
       thresholds and min_peak_dist are read here.
+    * `st = ann.open_ragged_stream(n_stations)`: the same with stations that advance at different rates
+      (`st.push([chunk_s (C, n_s) per station])`, `st.close()`, RaggedStream).
     Only the seist_*_dpk models (a [det, P, S] probability head) are supported."""
 
     def __init__(self, model, window: int = 8192, stride: int | None = None, batch: int = 256, norm_mode: str = "std",
@@ -474,6 +855,12 @@ class ContinuousAnnotator:
         if self.min_peak_dist is None or int(self.min_peak_dist) <= 1:
             raise ValueError(f"min_peak_dist must be > 1 samples, got {self.min_peak_dist}")
         return ContinuousStream(self, n_stations)
+
+    def open_ragged_stream(self, n_stations: int) -> RaggedStream:
+        """A stream whose stations advance at different rates (RaggedStream); thresholds and min_peak_dist are read here."""
+        if self.min_peak_dist is None or int(self.min_peak_dist) <= 1:
+            raise ValueError(f"min_peak_dist must be > 1 samples, got {self.min_peak_dist}")
+        return RaggedStream(self, n_stations)
 
     def pick_phases(self, probs: torch.Tensor, ppk_threshold: float | None = None, spk_threshold: float | None = None,
                     min_peak_dist: int | None = None):
