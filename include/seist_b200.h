@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 16
+#define SEIST_ABI_VERSION 17
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -475,6 +475,26 @@ int seist_ragged_runs_fill(const float* ext, const int64_t* ext_off, int32_t S, 
                            const int64_t* lo, const int64_t* hi, int64_t max_span, float threshold, const int64_t* g0,
                            const int64_t* open_in, int64_t* open_out, const void* work, int64_t work_bytes,
                            const int64_t* offsets, int64_t* pairs, void* stream);
+
+/* ---- raw histories of a ragged characterised stream (DESIGN §4.20) ---------------------------------------------------
+   A packed history holds station s as a (C, len_s) block at C * off[s], len_s = off[s + 1] - off[s], whose first sample
+   is the station's global sample h0[s]; off (S + 1,) and h0 (S,) are device int64 arrays, never read back to the host.
+   seist_ragged_history       = the packed counterpart of seist_stream_history: out row (s, c) = the samples
+                                [h0_out[s], h0_out[s] + len_out_s) of the held row (held_off, h0_held) followed by the
+                                station's block of the chunk packed as in SeistRaggedStep (chunk_off).  max_len >= every
+                                len_out_s sizes the grid (0 launches nothing); reads outside a station's own held and chunk
+                                blocks or past a buffer's capacity (floats) give 0.0f, writes past out_capacity are dropped.
+                                out overlaps neither input; S * C <= 65535.
+   seist_ragged_event_windows = seist_event_windows cutting from a packed history: station s the last one with
+                                offsets[s] <= e (a bounded search), p = index[e] - h0[s] rebased on the device, row s read at
+                                C * hist_off[s] with 0.0f outside [0, len_s) (and past hist_capacity).  Events >= M and
+                                picks outside the station's history give zero rows. */
+int seist_ragged_history(const float* held, const int64_t* held_off, const int64_t* h0_held, int64_t held_capacity, const float* chunk,
+                         const int64_t* chunk_off, int64_t chunk_capacity, const int64_t* h0_out, const int64_t* out_off, int32_t S,
+                         int32_t C, int64_t max_len, float* out, int64_t out_capacity, void* stream);
+int seist_ragged_event_windows(const float* hist, const int64_t* hist_off, const int64_t* h0, int64_t hist_capacity, int32_t S,
+                               int32_t C, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0, int32_t B, int32_t W,
+                               int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

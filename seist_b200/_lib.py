@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 16
+ABI_VERSION = 17
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -254,6 +254,10 @@ def lib():
     L.seist_ragged_runs.argtypes = [P, P, I32, I32, I32, I64, P, P, I64, F32, P, P, P, I64, P, P]
     L.seist_ragged_runs_fill.restype = C.c_int
     L.seist_ragged_runs_fill.argtypes = [P, P, I32, I32, I32, I64, P, P, I64, F32, P, P, P, P, I64, P, P, P]
+    L.seist_ragged_history.restype = C.c_int
+    L.seist_ragged_history.argtypes = [P, P, P, I64, P, P, I64, P, P, I32, I32, I64, P, I64, P]
+    L.seist_ragged_event_windows.restype = C.c_int
+    L.seist_ragged_event_windows.argtypes = [P, P, P, I64, I32, I32, P, I64, P, I64, I32, I32, I32, I32, P, I32, P]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -291,6 +295,7 @@ EXPORTS = [
     "seist_stream_peaks_work_bytes", "seist_stream_peaks", "seist_stream_peaks_fill", "seist_stream_runs", "seist_stream_runs_fill",
     "seist_sizeof_ragged_step", "seist_ragged_window", "seist_ragged_stack", "seist_ragged_emit", "seist_ragged_keep", "seist_ragged_ext",
     "seist_ragged_peaks", "seist_ragged_peaks_fill", "seist_ragged_runs", "seist_ragged_runs_fill",
+    "seist_ragged_history", "seist_ragged_event_windows",
 ]
 
 

@@ -734,6 +734,65 @@ __global__ void __launch_bounds__(ST_NT) ragged_keep_kernel(SeistRaggedStep p, c
   if (i < keep) tail_out[(size_t)blockIdx.y * p.W + i] = rg_raw(p, tail, chunk, s, c, r0, r1, r1 - keep + i);
 }
 
+// ---- raw histories of a ragged characterised stream (DESIGN §4.20) -------------------------------------------------
+// Station s's history is a (C, len_s) block at C * off[s] of a packed buffer, len_s = off[s + 1] - off[s], its first
+// sample the global h0[s].  CTA (x, s * C + c): out row (s, c) = samples [h0_out[s], h0_out[s] + n_out) of the held row
+// (base h0_held[s]) followed by the station's chunk block; every read is range-checked against the station's own
+// counts and the buffer's capacity (0.0f outside), every write against out's capacity.
+__global__ void __launch_bounds__(ST_NT) ragged_history_kernel(const float* __restrict__ held, const long long* __restrict__ held_off,
+                                                               const long long* __restrict__ h0_held, long long held_cap,
+                                                               const float* __restrict__ chunk, const long long* __restrict__ chunk_off,
+                                                               long long chunk_cap, const long long* __restrict__ h0_out,
+                                                               const long long* __restrict__ out_off, int C, float* __restrict__ out,
+                                                               long long out_cap) {
+  const int s = blockIdx.y / C, c = blockIdx.y % C;
+  const long long o0 = out_off[s], n_out = out_off[s + 1] - o0;
+  const long long i = (long long)blockIdx.x * ST_NT + threadIdx.x;
+  if (i >= n_out) return;
+  const long long a0 = held_off[s], n_held = held_off[s + 1] - a0, b0 = chunk_off[s], n = chunk_off[s + 1] - b0;
+  const long long j = h0_out[s] - h0_held[s] + i;
+  const long long hi = C * a0 + c * n_held + j, ci = C * b0 + c * n + (j - n_held);
+  float v = 0.f;
+  if (j >= 0 && j < n_held && hi < held_cap) v = held[hi];
+  else if (j >= n_held && j - n_held < n && ci < chunk_cap) v = chunk[ci];
+  const long long w = C * o0 + c * n_out + i;
+  if (w < out_cap) out[w] = v;
+}
+
+// event_windows_kernel cutting from packed histories: p = index[e0 + b] - h0[s] in station s's row, 0.0f outside
+// [0, len_s); events >= M and picks outside the station's history give zero rows
+__global__ void __launch_bounds__(PR_NT) ragged_event_windows_kernel(const float* __restrict__ hist, const long long* __restrict__ hist_off,
+                                                                     const long long* __restrict__ h0, long long hist_cap, int S, int C,
+                                                                     const long long* __restrict__ index,
+                                                                     const long long* __restrict__ offsets, long long M, long long e0,
+                                                                     int W, int a, int mode, EventDst dst, int n_dst) {
+  extern __shared__ float rew_row[];                // [W]: the zero-filled history slice, normalised in place
+  const int b = blockIdx.x / C, c = blockIdx.x % C;
+  const long long e = e0 + b;
+  const size_t row = (size_t)blockIdx.x * W;
+  const int s = rg_find((const int64_t*)offsets, S, e);
+  const long long h = hist_off[s], len = hist_off[s + 1] - h;
+  const long long p = e < M ? index[e] - h0[s] : -1;
+  if (p < 0 || p >= len) {
+#pragma unroll
+    for (int d = 0; d < EW_MAX_DST; ++d)
+      if (d < n_dst)
+        for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = 0.f;
+    return;
+  }
+  const long long src = C * h + c * len, t0 = p - a;
+  for (int i = threadIdx.x; i < W; i += PR_NT) {
+    const long long t = t0 + i;
+    rew_row[i] = t >= 0 && t < len && src + t < hist_cap ? hist[src + t] : 0.f;
+  }
+  __syncthreads();
+  pr_normalize_row(rew_row, rew_row, W, mode);
+#pragma unroll
+  for (int d = 0; d < EW_MAX_DST; ++d)
+    if (d < n_dst)
+      for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = rew_row[i];
+}
+
 // channel ch of row s of a packed ext, and its length
 __device__ __forceinline__ const float* rg_row(const float* ext, const long long* __restrict__ ext_off, int C, int ch, int s, long long& L) {
   const long long e0 = ext_off[s];
@@ -1379,6 +1438,51 @@ int seist_ragged_keep(const SeistRaggedStep* step, const float* tail_raw, const 
   ragged_keep_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(*step, tail_raw, chunk, tail_out);
   note_launch();
   return check_launch("ragged_keep");
+}
+
+int seist_ragged_history(const float* held, const int64_t* held_off, const int64_t* h0_held, int64_t held_capacity, const float* chunk,
+                         const int64_t* chunk_off, int64_t chunk_capacity, const int64_t* h0_out, const int64_t* out_off, int32_t S,
+                         int32_t C, int64_t max_len, float* out, int64_t out_capacity, void* stream) {
+  if (!held || !held_off || !h0_held || !chunk || !chunk_off || !h0_out || !out_off || !out || out == held || out == chunk || S <= 0 ||
+      C <= 0 || (long long)S * C > 65535 || held_capacity < 0 || chunk_capacity < 0 || out_capacity < 0 || max_len < 0 ||
+      max_len > INT32_MAX) {
+    set_error("ragged_history: bad arguments (non-null buffers and per-station arrays, out distinct from held and chunk, "
+              "S * C <= 65535, 0 <= max_len < 2^31, capacities >= 0)");
+    return -1;
+  }
+  if (max_len == 0) return 0;
+  const dim3 grid((unsigned)((max_len + ST_NT - 1) / ST_NT), (unsigned)(S * C));
+  ragged_history_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(
+      held, (const long long*)held_off, (const long long*)h0_held, held_capacity, chunk, (const long long*)chunk_off, chunk_capacity,
+      (const long long*)h0_out, (const long long*)out_off, C, out, out_capacity);
+  note_launch();
+  return check_launch("ragged_history");
+}
+
+int seist_ragged_event_windows(const float* hist, const int64_t* hist_off, const int64_t* h0, int64_t hist_capacity, int32_t S,
+                               int32_t C, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0, int32_t B, int32_t W,
+                               int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream) {
+  bool ok = hist && hist_off && h0 && hist_capacity >= 0 && (index || M == 0) && offsets && x && S > 0 && C > 0 && M >= 0 &&
+            e0 >= 0 && B > 0 && (long long)B * C <= INT32_MAX && W >= 1 && W <= 49152 && anchor >= 0 && anchor <= W && mode >= 0 &&
+            mode <= 2 && n_dst >= 1 && n_dst <= EW_MAX_DST;
+  EventDst dst{};
+  for (int d = 0; ok && d < n_dst; ++d) ok = (dst.x[d] = x[d]) != nullptr;
+  if (!ok) {
+    set_error("ragged_event_windows: bad arguments (non-null history and per-station arrays, 1 <= W <= 49152, 0 <= anchor <= W, "
+              "M >= 0, e0 >= 0, B > 0, mode 0 none, 1 std, 2 max, 1 to 4 non-null destinations)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(ragged_event_windows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  ragged_event_windows_kernel<<<(unsigned)((long long)B * C), PR_NT, smem, (cudaStream_t)stream>>>(
+      hist, (const long long*)hist_off, (const long long*)h0, hist_capacity, S, C, (const long long*)index, (const long long*)offsets, M,
+      e0, W, anchor, mode, dst, n_dst);
+  note_launch();
+  return check_launch("ragged_event_windows");
 }
 
 int seist_ragged_ext(const float* look, const float* probs, const int64_t* prob_off, const int64_t* ext_off, int32_t S, int32_t C,

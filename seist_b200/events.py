@@ -15,11 +15,12 @@ from __future__ import annotations
 import ctypes
 from typing import NamedTuple
 
+import numpy as np
 import torch
 
 from . import _lib
 from .infer import InferenceGraph
-from .stream import _I32_MAX, _MODES, ContinuousAnnotator, StreamOutput, _dense, _s
+from .stream import _I32_MAX, _MODES, ContinuousAnnotator, RaggedStreamOutput, StreamOutput, _dense, _flat, _prefix, _s, _upload
 
 MAX_MODELS = 4              # destinations of one seist_event_windows launch
 MAX_WINDOW = 49152          # a row of the window is staged in shared memory
@@ -133,12 +134,16 @@ class EventCharacterizer:
         return self._run(record.contiguous(), index, offsets)
 
     def _run(self, record: torch.Tensor, index: torch.Tensor, offsets: torch.Tensor) -> dict:
-        M = index.numel()
+        return self._batches(index.numel(), lambda xs, e0: event_windows_(xs, record, index, offsets, e0, self.window, self.anchor,
+                                                                          self.norm_mode))
+
+    def _batches(self, M: int, cut) -> dict:
+        """M events in batches: cut(xs, e0) writes every model's input for events e0 .., then each model replays."""
         out = {name: torch.empty((M,) if self.heads[name] == "reg" else (M, g.y.shape[1]), dtype=torch.float32, device=self.device)
                for name, g in self.graphs.items()}
         xs = [g.x for g in self.graphs.values()]
         for e0 in range(0, M, self.batch):
-            event_windows_(xs, record, index, offsets, e0, self.window, self.anchor, self.norm_mode)
+            cut(xs, e0)
             n = min(self.batch, M - e0)
             for name, g in self.graphs.items():
                 y = g.replay()
@@ -149,6 +154,11 @@ class EventCharacterizer:
         """A record picked chunk by chunk by `annotator` (a dpk ContinuousAnnotator, thresholds and min_peak_dist set),
         every P pick characterised in the call that emits it (DESIGN §4.18)."""
         return CharacterizedStream(self, annotator, n_stations)
+
+    def open_ragged_stream(self, annotator: ContinuousAnnotator, n_stations: int) -> "RaggedCharacterizedStream":
+        """Stations that advance at different rates (`annotator.open_ragged_stream`), every P pick characterised in the call
+        that emits it (DESIGN §4.20)."""
+        return RaggedCharacterizedStream(self, annotator, n_stations)
 
 
 def stream_history_(out: torch.Tensor, held: torch.Tensor, h0_held: int, chunk: torch.Tensor | None, h0_out: int) -> torch.Tensor:
@@ -169,6 +179,18 @@ def stream_history_(out: torch.Tensor, held: torch.Tensor, h0_held: int, chunk: 
     return out[:S * C * n_out].view(S, C, n_out)
 
 
+def _check_pair(ch: EventCharacterizer, ann: ContinuousAnnotator):
+    """A characteriser and an annotator that can stream together (raises ValueError otherwise)."""
+    dev = next(ann.model.parameters()).device
+    if dev != ch.device:
+        raise ValueError(f"the annotator's model is on {dev}, the characteriser's models on {ch.device}")
+    if ann.in_channels != ch.in_channels:
+        raise ValueError(f"the annotator takes {ann.in_channels} channels, the characteriser's models {ch.in_channels}")
+    if ch.window - ch.anchor > ann.window:
+        raise ValueError(f"the characteriser's window reaches {ch.window - ch.anchor} samples past the pick, more than the "
+                         f"annotator's window ({ann.window}): a pick's event window would not be pushed yet when it closes")
+
+
 class CharacterizedOutput(NamedTuple):
     """One call of a CharacterizedStream: the stream's StreamOutput and {name: outputs} for its P picks, row i for pick i
     of `out.ppk` ((m, classes) probabilities of a classification model, (m,) of a regression model)."""
@@ -185,14 +207,7 @@ class CharacterizedStream:
     no pick emitted since then starts its window.  `held_samples` = R - h0."""
 
     def __init__(self, ch: EventCharacterizer, ann: ContinuousAnnotator, n_stations: int):
-        dev = next(ann.model.parameters()).device
-        if dev != ch.device:
-            raise ValueError(f"the annotator's model is on {dev}, the characteriser's models on {ch.device}")
-        if ann.in_channels != ch.in_channels:
-            raise ValueError(f"the annotator takes {ann.in_channels} channels, the characteriser's models {ch.in_channels}")
-        if ch.window - ch.anchor > ann.window:
-            raise ValueError(f"the characteriser's window reaches {ch.window - ch.anchor} samples past the pick, more than the "
-                             f"annotator's window ({ann.window}): a pick's event window would not be pushed yet when it closes")
+        _check_pair(ch, ann)
         self.ch = ch
         self.stream = ann.open_stream(n_stations)
         self.S, self.C, self.device = self.stream.S, self.stream.C, self.stream.device
@@ -238,3 +253,150 @@ class CharacterizedStream:
         index, _, offsets = out.ppk
         rel = index - self.h0 if index.numel() else index
         return CharacterizedOutput(out, self.ch._run(self.history, rel, offsets))
+
+
+# ---- ragged characterised streams: stations that advance at different rates (DESIGN §4.20) ----------------------------
+def ragged_history_plan(h0, R, n, keep) -> dict:
+    """The per-station history bookkeeping of one call of a RaggedCharacterizedStream, from the held samples [h0, R) of
+    each station (S,), this call's push lengths n (S,) and the retention bounds keep (S,) of the previous call: a station
+    with n > 0 holds [keep, R + n) after the call, one with n = 0 keeps [h0, R).  Returns numpy int64 arrays h0, R, len
+    (S,) of the new histories and off (S + 1,), their exclusive prefix (station s packed as a (C, len) block at C * off[s])."""
+    h0, R, n, keep = (np.asarray(v, dtype=np.int64).reshape(-1) for v in (h0, R, n, keep))
+    if not (h0.shape == R.shape == n.shape == keep.shape) or (n < 0).any() or (h0 > R).any():
+        raise ValueError(f"expected (S,) counts with h0 <= R and n >= 0, got h0 {h0.tolist()}, R {R.tolist()}, n {n.tolist()}")
+    r1 = R + n
+    h0_out = np.where(n > 0, keep, h0)
+    if ((n > 0) & ((keep < h0) | (keep > r1))).any():
+        raise ValueError(f"a retention bound outside the held samples: h0 {h0.tolist()}, keep {keep.tolist()}, R + n {r1.tolist()}")
+    length = r1 - h0_out
+    return {"h0": h0_out, "R": r1, "len": length, "off": _prefix(length)}
+
+
+def _per_station(t: torch.Tensor, n: int, what: str, device):
+    if not (t.is_cuda and t.dtype == torch.int64 and t.dim() == 1 and t.is_contiguous() and t.numel() == n and t.device == device):
+        raise ValueError(f"{what}: expected a contiguous int64 CUDA tensor of shape ({n},) on {device}, "
+                         f"got {tuple(t.shape)} {t.dtype} on {t.device}")
+
+
+def ragged_history_(out: torch.Tensor, held: torch.Tensor, held_h0: torch.Tensor, held_off: torch.Tensor, chunk: torch.Tensor,
+                    chunk_off: torch.Tensor, h0_out: torch.Tensor, out_off: torch.Tensor, C: int, max_len: int) -> torch.Tensor:
+    """Write the packed histories (station s: samples [h0_out[s], ..) as a (C, len_s) block at C * out_off[s]) into the flat
+    float32 buffer out, from the packed held histories (held_h0, held_off) followed by each station's block of the packed
+    chunk (C * chunk_off[s]).  Per-station arrays are int64 on the device; max_len >= every len_s sizes the grid."""
+    S = h0_out.numel()
+    dev = held.device
+    _flat(held, 0, "held histories", dev)
+    _flat(chunk, 0, "packed chunk", dev)
+    _flat(out, 0, "history buffer", dev)
+    for t, what, k in ((held_h0, "held h0", S), (held_off, "held offsets", S + 1), (chunk_off, "chunk offsets", S + 1),
+                       (h0_out, "h0_out", S), (out_off, "out offsets", S + 1)):
+        _per_station(t, k, what, dev)
+    if not (S >= 1 and S * int(C) <= 65535 and 0 <= int(max_len) <= _I32_MAX):
+        raise ValueError(f"need 1 <= S, S * C <= 65535 and 0 <= max_len < 2^31, got S {S}, C {C}, max_len {max_len}")
+    if out.data_ptr() in (held.data_ptr(), chunk.data_ptr()):
+        raise ValueError("the history buffer must be distinct from the held histories and the chunk")
+    _lib.check(_lib.lib().seist_ragged_history(held.data_ptr(), held_off.data_ptr(), held_h0.data_ptr(), held.numel(), chunk.data_ptr(),
+                                               chunk_off.data_ptr(), chunk.numel(), h0_out.data_ptr(), out_off.data_ptr(), S, int(C),
+                                               int(max_len), out.data_ptr(), out.numel(), _s()), "seist_ragged_history")
+    return out
+
+
+def ragged_event_windows_(xs, hist: torch.Tensor, hist_h0: torch.Tensor, hist_off: torch.Tensor, index: torch.Tensor,
+                          offsets: torch.Tensor, e0: int, window: int, anchor: int, norm_mode: str = "std"):
+    """event_windows_ cutting from packed histories (station s: a (C, len_s) block at C * hist_off[s] whose first sample is
+    the global hist_h0[s]): every x in xs (B, C, window) gets events e0 .. e0 + B - 1 of the pick CSR, whose global
+    indices are rebased on the device; zeros outside the station's history."""
+    S = hist_h0.numel()
+    dev = hist.device
+    _flat(hist, 0, "histories", dev)
+    _per_station(hist_h0, S, "history h0", dev)
+    _per_station(hist_off, S + 1, "history offsets", dev)
+    if not 1 <= len(xs) <= MAX_MODELS:
+        raise ValueError(f"1 to {MAX_MODELS} destinations, got {len(xs)}")
+    C = xs[0].shape[1] if xs[0].dim() == 3 else -1
+    for x in xs:
+        _dense(x, (xs[0].shape[0], C, window), "event window batch", dev)
+    _check_picks(index, offsets, S, dev)
+    if not (1 <= window <= MAX_WINDOW and 0 <= anchor <= window and e0 >= 0 and S >= 1):
+        raise ValueError(f"need 1 <= window <= {MAX_WINDOW}, 0 <= anchor <= window and e0 >= 0, got window {window}, "
+                         f"anchor {anchor}, e0 {e0}")
+    ptrs = (ctypes.c_void_p * MAX_MODELS)(*[x.data_ptr() for x in xs])
+    _lib.check(_lib.lib().seist_ragged_event_windows(hist.data_ptr(), hist_off.data_ptr(), hist_h0.data_ptr(), hist.numel(), S, C,
+                                                     index.data_ptr(), index.numel(), offsets.data_ptr(), e0, xs[0].shape[0], window,
+                                                     anchor, _MODES[norm_mode], ptrs, len(xs), _s()), "seist_ragged_event_windows")
+    return xs
+
+
+class RaggedCharacterizedOutput(NamedTuple):
+    """One call of a RaggedCharacterizedStream: the RaggedStream's RaggedStreamOutput and {name: outputs} for its P picks,
+    row i for pick i of `out.ppk`."""
+    out: RaggedStreamOutput
+    events: dict
+
+
+class RaggedCharacterizedStream:
+    """`EventCharacterizer.open_ragged_stream(annotator, n_stations)`: `push(chunks)` with S float32 (C, n_s) tensors, any
+    n_s >= 0, then `close()`, each -> RaggedCharacterizedOutput.  Station s's events, concatenated over the calls, equal
+    `ch(rec_s[None], annotator.pick_phases(annotator.annotate(rec_s[None]))["ppk"])` of its own record bit for bit, each in
+    the call that emits its pick (DESIGN §4.20).  Each station keeps the §4.18 history on its own counts: the raw samples
+    [h0_s, R_s), h0_s the retention bound max(0, min(first pending P candidate, F_s - 1) - anchor) of the call before the
+    station's last non-empty push.  The histories are packed back to back in one of two flat device buffers, their h0 and
+    offsets in a small device array.  `held_samples` = R - h0 per station ((S,) int64)."""
+
+    def __init__(self, ch: EventCharacterizer, ann: ContinuousAnnotator, n_stations: int):
+        _check_pair(ch, ann)
+        self.ch = ch
+        self.stream = ann.open_ragged_stream(n_stations)
+        self.S, self.C, self.device = self.stream.S, self.stream.C, self.stream.device
+        self.buf = [torch.zeros(1, device=self.device), torch.zeros(1, device=self.device)]
+        self.desc = torch.zeros(2 * self.S + 1, dtype=torch.int64, device=self.device)   # h0 (S,), off (S + 1,) of buf[0]
+        self.h0 = np.zeros(self.S, np.int64)
+        self.R = np.zeros(self.S, np.int64)
+        self.keep = np.zeros(self.S, np.int64)       # the retention bounds after the last call
+
+    @property
+    def closed(self) -> bool:
+        return self.stream.closed
+
+    @property
+    def forwards(self) -> int:
+        return self.stream.forwards
+
+    @property
+    def held_samples(self) -> np.ndarray:
+        return self.R - self.h0
+
+    @torch.no_grad()
+    def push(self, chunks) -> RaggedCharacterizedOutput:
+        plan, chunk = self.stream._prepare(chunks)                # validates the chunks before any launch
+        n = plan["r1"] - plan["r0"]
+        hp = ragged_history_plan(self.h0, self.R, n, self.keep)
+        if (hp["len"] > _I32_MAX).any():
+            s = np.nonzero(hp["len"] > _I32_MAX)[0].tolist()
+            raise ValueError(f"the histories of stations {s} would hold {hp['len'][s].tolist()} samples, more than 2^31 - 1")
+        out = self.stream._call(plan, chunk, False)
+        if n.any():
+            S = self.S
+            need = self.C * int(hp["off"][-1])
+            if self.buf[1].numel() < need:
+                self.buf[1] = torch.empty(max(need, 2 * self.buf[1].numel()), device=self.device)
+            dev = _upload(np.concatenate([hp["h0"], hp["off"], plan["chunk_off"]]), self.device)   # the history descriptors
+            ragged_history_(self.buf[1], self.buf[0], self.desc[:S], self.desc[S:], chunk, dev[2 * S + 1:], dev[:S], dev[S:2 * S + 1],
+                            self.C, int(hp["len"].max()))
+            self.buf.reverse()
+            self.desc = dev[:2 * S + 1]
+            self.h0 = hp["h0"]
+        self.R = hp["R"]
+        return self._finish(out)
+
+    @torch.no_grad()
+    def close(self) -> RaggedCharacterizedOutput:
+        return self._finish(self.stream.close())
+
+    def _finish(self, out: RaggedStreamOutput) -> RaggedCharacterizedOutput:
+        pk, ch, S = self.stream.picker, self.ch, self.S
+        self.keep = np.maximum(self.keep, np.minimum(pk.first_pend[1], pk.F - 1) - ch.anchor)
+        index, _, offsets = out.ppk
+        hist, h0, off = self.buf[0], self.desc[:S], self.desc[S:]
+        return RaggedCharacterizedOutput(out, ch._batches(index.numel(), lambda xs, e0: ragged_event_windows_(
+            xs, hist, h0, off, index, offsets, e0, ch.window, ch.anchor, ch.norm_mode)))

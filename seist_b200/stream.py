@@ -728,6 +728,10 @@ class RaggedStream:
 
     @torch.no_grad()
     def push(self, chunks) -> RaggedStreamOutput:
+        return self._call(*self._prepare(chunks), False)
+
+    def _prepare(self, chunks):
+        """Validate a push (raises before any launch) -> (the call's plan, the chunks packed at C * chunk_off[s])."""
         if self.closed:
             raise RuntimeError("push() after close()")
         if len(chunks) != self.S:
@@ -743,7 +747,7 @@ class RaggedStream:
                 raise ValueError(f"station {s}: the chunk must be contiguous")
         plan = ragged_plan(self.R, [c.shape[1] for c in chunks], self.ann.window, self.ann.stride)
         chunk = torch.cat([c.reshape(-1) for c in chunks]) if plan["chunk_off"][-1] else self._none
-        return self._call(plan, chunk, False)
+        return plan, chunk
 
     @torch.no_grad()
     def close(self) -> RaggedStreamOutput:
