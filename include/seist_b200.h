@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 17
+#define SEIST_ABI_VERSION 18
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -495,6 +495,47 @@ int seist_ragged_history(const float* held, const int64_t* held_off, const int64
 int seist_ragged_event_windows(const float* hist, const int64_t* hist_off, const int64_t* h0, int64_t hist_capacity, int32_t S,
                                int32_t C, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0, int32_t B, int32_t W,
                                int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream);
+
+/* ---- whole records with data gaps (DESIGN §4.21) ----------------------------------------------------------------------
+   Sample t of station s is a gap sample when any channel of record (S, C, T) is not finite; a segment is a maximal run of
+   non-gap samples, inclusive [on, off].  The segment table: pairs (G, 2) int64 in station order then time order, seg_off
+   (S + 1,) int64 (station s holds segments seg_off[s] .. seg_off[s + 1] - 1), station (G,) int64.  A segment of at least
+   W samples is annotated: its windows are those of a record of off - on + 1 samples (K_g of them), packed back to back
+   over all segments by win_off (G + 1,) int64 (K_g = 0 for a short segment).  Every table read is range-checked: a
+   malformed table gives wrong output but no out-of-range access.
+   seist_gap_segments          = per station, the number of segments (counts (S,) int64) and, in work
+                                 (seist_runs_work_bytes(S, T)), per-block offsets for seist_gap_segments_fill, which
+                                 writes pairs for offsets = the exclusive prefix of counts (rows >= capacity are dropped).
+   seist_segment_window        = seist_window_batch over the packed windows j0 .. j0 + B - 1 (zero rows from n_win on):
+                                 window j is window j - win_off[g] of segment g (the last with win_off[g] <= j), cut in
+                                 place from the record at on_g + its start.
+   seist_segment_stack         = seist_stack_batch of those windows' outputs into probs (S, 3, T) at each segment's
+                                 samples; g0 .. g1 are the segments of windows j0 .. min(j0 + B, n_win) - 1.  Call with
+                                 j0 = 0, B, 2B, ... in order.
+   seist_segment_finish        = mode 0 (mean): divide every sample of an annotated segment by its number of covering
+                                 windows in the segment; both modes: NaN at every sample outside an annotated segment.
+   seist_segment_gather        = flat row r (a (3, m_r) block at 3 * prob_off[r], m_r = prob_off[r + 1] - prob_off[r]) =
+                                 probs[station, :, on + i] of segment rows[r], i < m_r; writes past capacity are dropped.
+   seist_segment_event_windows = seist_event_windows with the zero fill outside the pick's own segment: the segment of
+                                 station s holding p when annotated[g] (one byte each) is set, else a zero row. */
+int seist_gap_segments(const float* record, int32_t S, int32_t C, int64_t T, void* work, int64_t work_bytes, int64_t* counts,
+                       void* stream);
+int seist_gap_segments_fill(const float* record, int32_t S, int32_t C, int64_t T, const void* work, int64_t work_bytes,
+                            const int64_t* offsets, int64_t* pairs, int64_t capacity, void* stream);
+int seist_segment_window(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* pairs, const int64_t* station,
+                         const int64_t* win_off, int32_t G, int64_t n_win, int32_t W, int32_t P, int64_t j0, int32_t B, int32_t mode,
+                         float* x, void* stream);
+int seist_segment_stack(const float* y, int32_t S, int64_t T, const int64_t* pairs, const int64_t* station, const int64_t* win_off,
+                        int32_t G, int64_t n_win, int32_t W, int32_t P, int64_t j0, int32_t B, int32_t g0, int32_t g1, int32_t mode,
+                        float* probs, void* stream);
+int seist_segment_finish(float* probs, int32_t S, int64_t T, const int64_t* pairs, const int64_t* seg_off, int32_t G, int32_t W,
+                         int32_t P, int32_t mode, void* stream);
+int seist_segment_gather(const float* probs, int32_t S, int64_t T, const int64_t* pairs, const int64_t* station, int32_t G,
+                         const int64_t* rows, const int64_t* prob_off, int32_t n_rows, int64_t max_len, float* flat, int64_t capacity,
+                         void* stream);
+int seist_segment_event_windows(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* pairs, const int64_t* seg_off,
+                                const uint8_t* annotated, int32_t G, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0,
+                                int32_t B, int32_t W, int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 17
+ABI_VERSION = 18
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -258,6 +258,20 @@ def lib():
     L.seist_ragged_history.argtypes = [P, P, P, I64, P, P, I64, P, P, I32, I32, I64, P, I64, P]
     L.seist_ragged_event_windows.restype = C.c_int
     L.seist_ragged_event_windows.argtypes = [P, P, P, I64, I32, I32, P, I64, P, I64, I32, I32, I32, I32, P, I32, P]
+    L.seist_gap_segments.restype = C.c_int
+    L.seist_gap_segments.argtypes = [P, I32, I32, I64, P, I64, P, P]
+    L.seist_gap_segments_fill.restype = C.c_int
+    L.seist_gap_segments_fill.argtypes = [P, I32, I32, I64, P, I64, P, P, I64, P]
+    L.seist_segment_window.restype = C.c_int
+    L.seist_segment_window.argtypes = [P, I32, I32, I64, P, P, P, I32, I64, I32, I32, I64, I32, I32, P, P]
+    L.seist_segment_stack.restype = C.c_int
+    L.seist_segment_stack.argtypes = [P, I32, I64, P, P, P, I32, I64, I32, I32, I64, I32, I32, I32, I32, P, P]
+    L.seist_segment_finish.restype = C.c_int
+    L.seist_segment_finish.argtypes = [P, I32, I64, P, P, I32, I32, I32, I32, P]
+    L.seist_segment_gather.restype = C.c_int
+    L.seist_segment_gather.argtypes = [P, I32, I64, P, P, I32, P, P, I32, I64, P, I64, P]
+    L.seist_segment_event_windows.restype = C.c_int
+    L.seist_segment_event_windows.argtypes = [P, I32, I32, I64, P, P, P, I32, P, I64, P, I64, I32, I32, I32, I32, P, I32, P]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -296,6 +310,8 @@ EXPORTS = [
     "seist_sizeof_ragged_step", "seist_ragged_window", "seist_ragged_stack", "seist_ragged_emit", "seist_ragged_keep", "seist_ragged_ext",
     "seist_ragged_peaks", "seist_ragged_peaks_fill", "seist_ragged_runs", "seist_ragged_runs_fill",
     "seist_ragged_history", "seist_ragged_event_windows",
+    "seist_gap_segments", "seist_gap_segments_fill", "seist_segment_window", "seist_segment_stack", "seist_segment_finish",
+    "seist_segment_gather", "seist_segment_event_windows",
 ]
 
 

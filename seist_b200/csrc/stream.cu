@@ -983,6 +983,225 @@ __global__ void __launch_bounds__(ST_NT) rg_srun_fill_kernel(const float* __rest
   }
 }
 
+// ---- whole records with data gaps (DESIGN §4.21) --------------------------------------------------------------------
+// A sample is usable when every channel is finite; a segment is a maximal run of usable samples.  Each thread tests its
+// own sample and takes its neighbour's verdict from the next lane, so a pass reads every sample of the record once.
+__device__ __forceinline__ bool gp_ok(const float* x, int C, long long T, long long t) {
+  bool ok = true;
+  for (int c = 0; c < C; ++c) ok = ok && isfinite(x[(size_t)c * T + t]);
+  return ok;
+}
+
+// blocks of ST_CH samples; blk (S, nblk): the segment starts of each block
+__global__ void __launch_bounds__(ST_NT) gap_count_kernel(const float* __restrict__ rec, int C, int T, int* __restrict__ blk, int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = rec + (size_t)blockIdx.y * C * T;
+  const int a = blockIdx.x * ST_CH, e = min(a + ST_CH, T), lane = threadIdx.x & 31;
+  int n = 0;
+  for (int i0 = a; i0 < e; i0 += ST_NT) {
+    const int i = i0 + threadIdx.x;
+    const bool ok = i < e && gp_ok(x, C, T, i);
+    bool prev = __shfl_up_sync(0xffffffffu, ok, 1);
+    if (lane == 0) prev = i > 0 && i < e && gp_ok(x, C, T, i - 1);
+    n += ok && !prev;
+  }
+  n = st_block_count(n, warp_s);
+  if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
+}
+
+// run_fill_kernel with usable / not usable for p > thr: blk holds the exclusive start offsets per block, the ends before a
+// block are as many, less one when a segment crosses into it; rows >= cap are dropped
+__global__ void __launch_bounds__(ST_NT) gap_fill_kernel(const float* __restrict__ rec, int C, int T, const int* __restrict__ blk,
+                                                         int nblk, const long long* __restrict__ offsets, long long cap,
+                                                         long long* __restrict__ pairs) {
+  __shared__ int warp_s[ST_NT / 32];
+  const float* x = rec + (size_t)blockIdx.y * C * T;
+  const int a = blockIdx.x * ST_CH, e = min(a + ST_CH, T), lane = threadIdx.x & 31;
+  const long long b0 = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  long long on_base = b0, off_base = b0 - (a > 0 && gp_ok(x, C, T, a - 1) && gp_ok(x, C, T, a) ? 1 : 0);
+  for (int i0 = a; i0 < e; i0 += ST_NT) {
+    const int i = i0 + threadIdx.x;
+    const bool ok = i < e && gp_ok(x, C, T, i);
+    bool prev = __shfl_up_sync(0xffffffffu, ok, 1), next = __shfl_down_sync(0xffffffffu, ok, 1);
+    if (lane == 0) prev = i > 0 && i < e && gp_ok(x, C, T, i - 1);
+    if (lane == 31) next = i + 1 < T && gp_ok(x, C, T, i + 1);   // i + 1 < e for every other lane of a full warp
+    const bool fon = ok && !prev, foff = ok && (i == T - 1 || !next);
+    int ton, toff;
+    const int ron = st_block_rank(fon, warp_s, ton);
+    const int roff = st_block_rank(foff, warp_s, toff);
+    if (fon && on_base + ron < cap) pairs[(on_base + ron) * 2] = i;
+    if (foff && off_base + roff >= 0 && off_base + roff < cap) pairs[(off_base + roff) * 2 + 1] = i;
+    on_base += ton;
+    off_base += toff;
+  }
+}
+
+// segment g of a table of G: its first sample, length and station when they describe an annotated segment of a record
+// (S, ., T) for windows of W, else false
+__device__ __forceinline__ bool sg_get(const long long* pairs, const long long* station, int G, int g, int S, long long T, int W,
+                                       long long& on, long long& len, int& s) {
+  if (g < 0 || g >= G) return false;
+  on = pairs[2 * (size_t)g];
+  len = pairs[2 * (size_t)g + 1] - on + 1;
+  const long long st = station[g];
+  s = (int)st;
+  return on >= 0 && len >= W && on + len <= T && st >= 0 && st < S;
+}
+
+// the segment of station s holding sample t: the last g in the station's range with on_g <= t, when t <= off_g; else -1
+__device__ __forceinline__ int sg_find(const long long* pairs, const long long* seg_off, int G, int s, long long t) {
+  const long long g0 = min(max(seg_off[s], 0LL), (long long)G), g1 = min(max(seg_off[s + 1], g0), (long long)G);
+  if (g0 >= g1 || pairs[2 * g0] > t) return -1;
+  long long lo = g0, hi = g1 - 1;
+  while (lo < hi) {
+    const long long mid = (lo + hi + 1) >> 1;
+    if (pairs[2 * mid] <= t) lo = mid; else hi = mid - 1;
+  }
+  return t <= pairs[2 * lo + 1] ? (int)lo : -1;
+}
+
+// x (B, C, W): row (b, c) = normalised record[s, c, on + start(q) : + W] for packed window j0 + b = window q of segment g
+__global__ void __launch_bounds__(PR_NT) segment_window_kernel(const float* __restrict__ rec, int S, int C, long long T,
+                                                               const long long* __restrict__ pairs, const long long* __restrict__ station,
+                                                               const long long* __restrict__ win_off, int G, long long n_win, int W,
+                                                               int P, long long j0, int mode, float* __restrict__ x) {
+  extern __shared__ float sg_row[];                 // [W]: the record slice, read from global memory once
+  const int b = blockIdx.x / C, c = blockIdx.x % C;
+  const long long j = j0 + b;
+  float* dst = x + (size_t)blockIdx.x * W;
+  long long a = -1, on, len;
+  int s = 0;
+  if (j < n_win) {
+    const int g = rg_find((const int64_t*)win_off, G, j);
+    const long long q = j - win_off[g];
+    if (sg_get(pairs, station, G, g, S, T, W, on, len, s) && q >= 0) {
+      const Windows win((int)len, W, P);
+      if (q < win.K) a = on + win.start((int)q);
+    }
+  }
+  if (a < 0) {
+    for (int i = threadIdx.x; i < W; i += PR_NT) dst[i] = 0.f;
+    return;
+  }
+  const float* src = rec + ((size_t)s * C + c) * T + a;
+  for (int i = threadIdx.x; i < W; i += PR_NT) sg_row[i] = src[i];
+  __syncthreads();
+  pr_normalize_row(sg_row, dst, W, mode);
+}
+
+// stack_batch_kernel per segment: CTA (x, g - g0, c) gathers the batch's windows of segment g into probs[s, c, on + t]
+__global__ void __launch_bounds__(ST_NT) segment_stack_kernel(const float* __restrict__ y, int S, long long T,
+                                                              const long long* __restrict__ pairs, const long long* __restrict__ station,
+                                                              const long long* __restrict__ win_off, int G, int W, int P, long long j0,
+                                                              int nb, int g0, int mode, float* __restrict__ probs) {
+  const int g = g0 + blockIdx.y, c = blockIdx.z;
+  long long on, len;
+  int s;
+  if (!sg_get(pairs, station, G, g, S, T, W, on, len, s)) return;
+  const Windows win((int)len, W, P);
+  const long long wb = win_off[g];
+  const long long ka_ = max(j0 - wb, 0LL), kb_ = min(min(j0 + nb - 1 - wb, (long long)win.K - 1), win_off[g + 1] - wb - 1);
+  if (ka_ > kb_) return;
+  const int ka = (int)ka_, kb = (int)kb_;
+  const int t = win.start(ka) + blockIdx.x * ST_NT + threadIdx.x;
+  if (t >= win.start(kb) + W) return;
+  int lo, hi;
+  bool tail;
+  win.cover(t, lo, hi, tail);
+  const int first = lo <= hi ? lo : win.K - 1;
+  float* out = probs + ((size_t)s * 3 + c) * T + on + t;
+  float acc = first >= ka ? (mode == 0 ? 0.f : -INFINITY) : *out;
+  const float* yb = y + (size_t)c * W;
+  for (int k = max(lo, ka); k <= min(hi, kb); ++k) {
+    const float v = yb[(size_t)(wb + k - j0) * 3 * W + (t - k * P)];
+    acc = mode == 0 ? acc + v : fmaxf(acc, v);
+  }
+  if (tail && win.K - 1 >= ka && win.K - 1 <= kb) {
+    const float v = yb[(size_t)(wb + win.K - 1 - j0) * 3 * W + (t - (win.T - W))];
+    acc = mode == 0 ? acc + v : fmaxf(acc, v);
+  }
+  *out = acc;
+}
+
+// mean: one IEEE division by the covering windows within the segment; NaN outside every annotated segment
+__global__ void __launch_bounds__(ST_NT) segment_finish_kernel(float* __restrict__ probs, int S, long long T,
+                                                               const long long* __restrict__ pairs, const long long* __restrict__ seg_off,
+                                                               int G, int W, int P, int mode, long long n) {
+  for (long long i = blockIdx.x * (long long)ST_NT + threadIdx.x; i < n; i += (long long)gridDim.x * ST_NT) {
+    const int s = (int)(i / (3 * T));
+    const long long t = i % T;
+    const int g = sg_find(pairs, seg_off, G, s, t);
+    const long long on = g >= 0 ? pairs[2 * (size_t)g] : 0, len = g >= 0 ? pairs[2 * (size_t)g + 1] - on + 1 : 0;
+    if (g < 0 || len < W || on < 0 || on + len > T) {
+      probs[i] = NAN;
+    } else if (mode == 0) {
+      int lo, hi;
+      bool tail;
+      Windows((int)len, W, P).cover((int)(t - on), lo, hi, tail);
+      const int cnt = max(hi - lo + 1, 0) + (tail ? 1 : 0);
+      probs[i] = __fdiv_rn(probs[i], (float)cnt);
+    }
+  }
+}
+
+// CTA (x, r, c): flat (3, m_r) block of row r at 3 * prob_off[r] = probs[s, c, on + i] of segment rows[r] (0.0f when the
+// row names no segment of the table or runs past the record)
+__global__ void __launch_bounds__(ST_NT) segment_gather_kernel(const float* __restrict__ probs, int S, long long T,
+                                                               const long long* __restrict__ pairs, const long long* __restrict__ station,
+                                                               int G, const long long* __restrict__ rows,
+                                                               const long long* __restrict__ prob_off, long long cap,
+                                                               float* __restrict__ flat) {
+  const int r = blockIdx.y, c = blockIdx.z;
+  const long long o0 = prob_off[r], m = prob_off[r + 1] - o0, i = blockIdx.x * (long long)ST_NT + threadIdx.x;
+  if (i >= m) return;
+  const long long g = rows[r];
+  float v = 0.f;
+  if (g >= 0 && g < G) {
+    const long long on = pairs[2 * g], st = station[g];
+    if (st >= 0 && st < S && on >= 0 && on + i < T) v = probs[((size_t)st * 3 + c) * T + on + i];
+  }
+  const long long w = 3 * o0 + c * m + i;
+  if (w >= 0 && w < cap) flat[w] = v;
+}
+
+// event_windows_kernel zero-filling outside the pick's own annotated segment [on, off]; picks outside every annotated
+// segment give zero rows
+__global__ void __launch_bounds__(PR_NT) segment_event_windows_kernel(const float* __restrict__ rec, int S, int C, long long T,
+                                                                      const long long* __restrict__ pairs,
+                                                                      const long long* __restrict__ seg_off,
+                                                                      const unsigned char* __restrict__ annotated, int G,
+                                                                      const long long* __restrict__ index,
+                                                                      const long long* __restrict__ offsets, long long M, long long e0,
+                                                                      int W, int a, int mode, EventDst dst, int n_dst) {
+  extern __shared__ float sew_row[];                // [W]: the zero-filled segment slice, normalised in place
+  const int b = blockIdx.x / C, c = blockIdx.x % C;
+  const long long e = e0 + b;
+  const size_t row = (size_t)blockIdx.x * W;
+  const long long p = e < M ? index[e] : -1;
+  const int s = rg_find((const int64_t*)offsets, S, e);
+  const int g = p >= 0 && p < T ? sg_find(pairs, seg_off, G, s, p) : -1;
+  const long long on = g >= 0 ? pairs[2 * (size_t)g] : 0, off = g >= 0 ? pairs[2 * (size_t)g + 1] : -1;
+  if (g < 0 || !annotated[g] || on < 0 || off >= T) {
+#pragma unroll
+    for (int d = 0; d < EW_MAX_DST; ++d)
+      if (d < n_dst)
+        for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = 0.f;
+    return;
+  }
+  const float* src = rec + ((size_t)s * C + c) * T;
+  const long long t0 = p - a;
+  for (int i = threadIdx.x; i < W; i += PR_NT) {
+    const long long t = t0 + i;
+    sew_row[i] = t >= on && t <= off ? src[t] : 0.f;
+  }
+  __syncthreads();
+  pr_normalize_row(sew_row, sew_row, W, mode);
+#pragma unroll
+  for (int d = 0; d < EW_MAX_DST; ++d)
+    if (d < n_dst)
+      for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = sew_row[i];
+}
+
 // ---- work buffers ---------------------------------------------------------------------------------------------------
 __host__ __device__ inline size_t st_align(size_t b) { return (b + 255) & ~(size_t)255; }
 inline int st_capc(int T) { return T / 2 + 1; }                 // candidates of a row: never two adjacent samples
@@ -1592,6 +1811,144 @@ int seist_ragged_runs_fill(const float* ext, const int64_t* ext_off, int32_t S, 
                                                                        (long long*)open_out, (long long*)pairs);
   note_launch();
   return check_launch("ragged_runs_fill");
+}
+
+int seist_gap_segments(const float* record, int32_t S, int32_t C, int64_t T, void* work, int64_t work_bytes, int64_t* counts,
+                       void* stream) {
+  if (!record || !work || !counts || S <= 0 || S > 65535 || C <= 0 || T < 1 || T > INT32_MAX || work_bytes < seist_runs_work_bytes(S, T)) {
+    set_error("gap_segments: bad arguments (1 <= T < 2^31, 1 <= S <= 65535, C >= 1, work >= seist_runs_work_bytes(S, T))");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int* total = (int*)work;
+  int* blk = (int*)((char*)work + st_align(sizeof(int) * S));
+  const int nblk = st_nblk((int)T);
+  gap_count_kernel<<<dim3(nblk, S), ST_NT, 0, st>>>(record, C, (int)T, blk, nblk);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(blk, nblk, total, (long long*)counts);
+  note_launch();
+  note_launch();
+  return check_launch("gap_segments");
+}
+
+int seist_gap_segments_fill(const float* record, int32_t S, int32_t C, int64_t T, const void* work, int64_t work_bytes,
+                            const int64_t* offsets, int64_t* pairs, int64_t capacity, void* stream) {
+  if (!record || !work || !offsets || !pairs || S <= 0 || S > 65535 || C <= 0 || T < 1 || T > INT32_MAX || capacity < 0 ||
+      work_bytes < seist_runs_work_bytes(S, T)) {
+    set_error("gap_segments_fill: bad arguments (the work buffer of the seist_gap_segments call, non-null pairs, capacity >= 0)");
+    return -1;
+  }
+  const int* blk = (const int*)((const char*)work + st_align(sizeof(int) * S));
+  const int nblk = st_nblk((int)T);
+  gap_fill_kernel<<<dim3(nblk, S), ST_NT, 0, (cudaStream_t)stream>>>(record, C, (int)T, blk, nblk, (const long long*)offsets, capacity,
+                                                                     (long long*)pairs);
+  note_launch();
+  return check_launch("gap_segments_fill");
+}
+
+static bool sg_ok(int32_t S, int64_t T, const int64_t* pairs, const int64_t* per_seg, int32_t G, int32_t W, int32_t P) {
+  return pairs && per_seg && S > 0 && S <= 65535 && T >= 1 && T <= INT32_MAX && G >= 1 && W >= 1 && W <= 49152 && P >= 1 && P <= W;
+}
+
+int seist_segment_window(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* pairs, const int64_t* station,
+                         const int64_t* win_off, int32_t G, int64_t n_win, int32_t W, int32_t P, int64_t j0, int32_t B, int32_t mode,
+                         float* x, void* stream) {
+  if (!sg_ok(S, T, pairs, station, G, W, P) || !record || !win_off || !x || C <= 0 || n_win < 0 || j0 < 0 || B <= 0 ||
+      (long long)B * C > INT32_MAX || mode < 0 || mode > 2) {
+    set_error("segment_window: bad arguments (1 <= T < 2^31, 1 <= S <= 65535, G >= 1, 1 <= P <= W <= 49152, n_win >= 0, j0 >= 0, "
+              "B > 0, mode 0 none, 1 std, 2 max)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(segment_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  segment_window_kernel<<<(unsigned)((long long)B * C), PR_NT, smem, (cudaStream_t)stream>>>(
+      record, S, C, T, (const long long*)pairs, (const long long*)station, (const long long*)win_off, G, n_win, W, P, j0, mode, x);
+  note_launch();
+  return check_launch("segment_window");
+}
+
+int seist_segment_stack(const float* y, int32_t S, int64_t T, const int64_t* pairs, const int64_t* station, const int64_t* win_off,
+                        int32_t G, int64_t n_win, int32_t W, int32_t P, int64_t j0, int32_t B, int32_t g0, int32_t g1, int32_t mode,
+                        float* probs, void* stream) {
+  if (!sg_ok(S, T, pairs, station, G, W, P) || !y || !win_off || !probs || n_win < 0 || j0 < 0 || B <= 0 || g0 < 0 || g1 < g0 ||
+      g1 >= G || mode < 0 || mode > 1) {
+    set_error("segment_stack: bad arguments (1 <= T < 2^31, 1 <= S <= 65535, 1 <= P <= W <= 49152, j0 >= 0, B > 0, "
+              "0 <= g0 <= g1 < G, mode 0 mean, 1 max)");
+    return -1;
+  }
+  if (j0 >= n_win) return 0;
+  const int nb = (int)std::min<long long>(B, n_win - j0);
+  const long long span = std::min<long long>(T, (long long)(nb - 1) * P + W);
+  // short segments between two annotated ones hold no windows but are rows of the grid: more than 65535 of them in one
+  // batch take more than one launch
+  for (int gs = g0; gs <= g1; gs += 65535) {
+    const dim3 grid((unsigned)((span + ST_NT - 1) / ST_NT), (unsigned)std::min(65535, g1 - gs + 1), 3);
+    segment_stack_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(y, S, T, (const long long*)pairs, (const long long*)station,
+                                                                   (const long long*)win_off, G, W, P, j0, nb, gs, mode, probs);
+    note_launch();
+    if (g1 - gs < 65535) break;
+  }
+  return check_launch("segment_stack");
+}
+
+int seist_segment_finish(float* probs, int32_t S, int64_t T, const int64_t* pairs, const int64_t* seg_off, int32_t G, int32_t W,
+                         int32_t P, int32_t mode, void* stream) {
+  if (!probs || !seg_off || S <= 0 || S > 65535 || T < 1 || T > INT32_MAX || G < 0 || (G > 0 && !pairs) || W < 1 || W > 49152 || P < 1 ||
+      P > W || mode < 0 || mode > 1) {
+    set_error("segment_finish: bad arguments (1 <= T < 2^31, 1 <= S <= 65535, G >= 0, 1 <= P <= W <= 49152, mode 0 mean, 1 max)");
+    return -1;
+  }
+  const long long n = (long long)S * 3 * T;
+  const long long g = std::min<long long>((n + ST_NT - 1) / ST_NT, 132LL * 16);
+  segment_finish_kernel<<<(unsigned)g, ST_NT, 0, (cudaStream_t)stream>>>(probs, S, T, (const long long*)pairs, (const long long*)seg_off,
+                                                                          G, W, P, mode, n);
+  note_launch();
+  return check_launch("segment_finish");
+}
+
+int seist_segment_gather(const float* probs, int32_t S, int64_t T, const int64_t* pairs, const int64_t* station, int32_t G,
+                         const int64_t* rows, const int64_t* prob_off, int32_t n_rows, int64_t max_len, float* flat, int64_t capacity,
+                         void* stream) {
+  if (!probs || !pairs || !station || !rows || !prob_off || !flat || S <= 0 || S > 65535 || T < 1 || T > INT32_MAX || G < 1 ||
+      n_rows < 1 || n_rows > 65535 || max_len < 0 || max_len > INT32_MAX || capacity < 0) {
+    set_error("segment_gather: bad arguments (1 <= T < 2^31, 1 <= S <= 65535, G >= 1, 1 <= n_rows <= 65535, 0 <= max_len < 2^31)");
+    return -1;
+  }
+  if (max_len == 0) return 0;
+  const dim3 grid((unsigned)((max_len + ST_NT - 1) / ST_NT), (unsigned)n_rows, 3);
+  segment_gather_kernel<<<grid, ST_NT, 0, (cudaStream_t)stream>>>(probs, S, T, (const long long*)pairs, (const long long*)station, G,
+                                                                  (const long long*)rows, (const long long*)prob_off, capacity, flat);
+  note_launch();
+  return check_launch("segment_gather");
+}
+
+int seist_segment_event_windows(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* pairs, const int64_t* seg_off,
+                                const uint8_t* annotated, int32_t G, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0,
+                                int32_t B, int32_t W, int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream) {
+  bool ok = record && seg_off && (G == 0 || (pairs && annotated)) && G >= 0 && (index || M == 0) && offsets && x && S > 0 &&
+            S <= 65535 && C > 0 && T >= 1 && T <= INT32_MAX && M >= 0 && e0 >= 0 && B > 0 && (long long)B * C <= INT32_MAX && W >= 1 &&
+            W <= 49152 && anchor >= 0 && anchor <= W && mode >= 0 && mode <= 2 && n_dst >= 1 && n_dst <= EW_MAX_DST;
+  EventDst dst{};
+  for (int d = 0; ok && d < n_dst; ++d) ok = (dst.x[d] = x[d]) != nullptr;
+  if (!ok) {
+    set_error("segment_event_windows: bad arguments (1 <= T < 2^31, 1 <= S <= 65535, G >= 0, 1 <= W <= 49152, 0 <= anchor <= W, "
+              "M >= 0, e0 >= 0, B > 0, mode 0 none, 1 std, 2 max, 1 to 4 non-null destinations)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(segment_event_windows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  segment_event_windows_kernel<<<(unsigned)((long long)B * C), PR_NT, smem, (cudaStream_t)stream>>>(
+      record, S, C, T, (const long long*)pairs, (const long long*)seg_off, annotated, G, (const long long*)index, (const long long*)offsets,
+      M, e0, W, anchor, mode, dst, n_dst);
+  note_launch();
+  return check_launch("segment_event_windows");
 }
 
 }  // extern "C"

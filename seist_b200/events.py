@@ -20,7 +20,8 @@ import torch
 
 from . import _lib
 from .infer import InferenceGraph
-from .stream import _I32_MAX, _MODES, ContinuousAnnotator, RaggedStreamOutput, StreamOutput, _dense, _flat, _prefix, _s, _upload
+from .stream import (_I32_MAX, _MODES, ContinuousAnnotator, RaggedStreamOutput, Segments, StreamOutput, _dense, _flat, _prefix, _s,
+                     _upload, check_segments)
 
 MAX_MODELS = 4              # destinations of one seist_event_windows launch
 MAX_WINDOW = 49152          # a row of the window is staged in shared memory
@@ -59,6 +60,30 @@ def event_windows_(xs, record: torch.Tensor, index: torch.Tensor, offsets: torch
     _lib.check(_lib.lib().seist_event_windows(record.data_ptr(), S, C, T, index.data_ptr(), index.numel(), offsets.data_ptr(), e0,
                                               xs[0].shape[0], window, anchor, _MODES[norm_mode], ptrs, len(xs), _s()),
                "seist_event_windows")
+    return xs
+
+
+def segment_event_windows_(xs, record: torch.Tensor, segs: Segments, index: torch.Tensor, offsets: torch.Tensor, e0: int, window: int,
+                           anchor: int, norm_mode: str = "std"):
+    """event_windows_ zero-filling outside the pick's own annotated segment of `segs` (gap_segments of record) instead of
+    outside [0, T); picks outside every annotated segment give zero rows."""
+    _dense(record, (None, None, None), "record")
+    S, C, T = record.shape
+    if not 1 <= len(xs) <= MAX_MODELS:
+        raise ValueError(f"1 to {MAX_MODELS} destinations, got {len(xs)}")
+    for x in xs:
+        _dense(x, (xs[0].shape[0], C, window), "event window batch", record.device)
+    _check_picks(index, offsets, S, record.device)
+    check_segments(segs, S, T, record.device)
+    if not (1 <= window <= MAX_WINDOW and 0 <= anchor <= window and T < 2 ** 31 and e0 >= 0):
+        raise ValueError(f"need 1 <= window <= {MAX_WINDOW}, 0 <= anchor <= window, T < 2^31 and e0 >= 0, got window {window}, "
+                         f"anchor {anchor}, T {T}, e0 {e0}")
+    G = len(segs.on)
+    ptrs = (ctypes.c_void_p * MAX_MODELS)(*[x.data_ptr() for x in xs])
+    _lib.check(_lib.lib().seist_segment_event_windows(record.data_ptr(), S, C, T, segs.pairs.data_ptr() if G else None,
+                                                      segs.offsets.data_ptr(), segs.annotated.data_ptr() if G else None, G,
+                                                      index.data_ptr(), index.numel(), offsets.data_ptr(), e0, xs[0].shape[0], window,
+                                                      anchor, _MODES[norm_mode], ptrs, len(xs), _s()), "seist_segment_event_windows")
     return xs
 
 
@@ -117,7 +142,9 @@ class EventCharacterizer:
         return cls(models, window=args.in_samples, p_position_ratio=args.p_position_ratio, norm_mode=args.norm_mode, **kwargs)
 
     @torch.no_grad()
-    def __call__(self, record: torch.Tensor, ppk) -> dict:
+    def __call__(self, record: torch.Tensor, ppk, segments: Segments | None = None) -> dict:
+        """With segments (`ContinuousAnnotator.segments(record)`), each pick's window is zero outside the pick's own
+        annotated segment, and a pick outside every annotated segment gets a zero window (DESIGN §4.21)."""
         index, offsets = ppk[0], ppk[-1]
         if not record.is_cuda or not index.is_cuda or not offsets.is_cuda:
             raise RuntimeError("EventCharacterizer has no CPU path: the record and the picks must live on the models' CUDA device")
@@ -131,6 +158,11 @@ class EventCharacterizer:
         if T >= 2 ** 31:
             raise ValueError(f"record length {T} must stay below 2^31 samples")
         _check_picks(index, offsets, S, self.device)
+        if segments is not None:
+            check_segments(segments, S, T, self.device)
+            record = record.contiguous()
+            return self._batches(index.numel(), lambda xs, e0: segment_event_windows_(
+                xs, record, segments, index, offsets, e0, self.window, self.anchor, self.norm_mode))
         return self._run(record.contiguous(), index, offsets)
 
     def _run(self, record: torch.Tensor, index: torch.Tensor, offsets: torch.Tensor) -> dict:

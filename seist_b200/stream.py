@@ -642,6 +642,12 @@ class RaggedPickStream:
         return np.concatenate(parts).astype(np.int64), meta
 
     def _run(self, flat: torch.Tensor, m: np.ndarray, last: bool, host: np.ndarray, dev: torch.Tensor, meta: dict):
+        staged = self._stage(flat, host, dev, meta)
+        return self._collect(staged, staged["totals"].tolist(), last)   # the one host sync
+
+    def _stage(self, flat: torch.Tensor, host: np.ndarray, dev: torch.Tensor, meta: dict) -> dict:
+        """Every launch of a call up to the host read: ext, both channels' peaks and the runs.  `totals` is the int64
+        device tensor that `_collect` needs on the host."""
         S, lib, d, max_L = self.S, _lib.lib(), self.device, meta["max_L"]
         ptr = dev.data_ptr()
         prob_off, ext_off = ptr, ptr + 8 * (S + 1)
@@ -674,7 +680,16 @@ class RaggedPickStream:
                                          self.open.data_ptr(), open_out.data_ptr(), rwork.data_ptr(), rbytes, rcounts.data_ptr(), _s()),
                    "seist_ragged_runs")
         roff = _offsets(rcounts)
-        tot = torch.cat([staged[0][2][-1:], staged[1][2][-1:], roff[-1:], staged[0][3], staged[1][3]]).tolist()   # the one host sync
+        totals = torch.cat([staged[0][2][-1:], staged[1][2][-1:], roff[-1:], staged[0][3], staged[1][3]])
+        return dict(staged=staged, totals=totals, meta=meta, chp=chp, ext=ext, ext_off=ext_off, rlo=rlo, rhi=rhi, g0=g0, rwork=rwork,
+                    rbytes=rbytes, roff=roff, open_out=open_out, look_out=look_out)
+
+    def _collect(self, st: dict, tot: list, last: bool):
+        """The rest of a call once its totals are on the host: the picks and runs that closed, and the carried state."""
+        S, lib, d = self.S, _lib.lib(), self.device
+        staged, meta, chp, ext, ext_off = st["staged"], st["meta"], st["chp"], st["ext"], st["ext_off"]
+        rlo, rhi, g0, rwork, rbytes, roff, open_out = st["rlo"], st["rhi"], st["g0"], st["rwork"], st["rbytes"], st["roff"], st["open_out"]
+        max_L = meta["max_L"]
         out = []
         for i, (ch, (work, capc, off, info)) in enumerate(zip((1, 2), staged)):
             n = tot[i]
@@ -693,7 +708,7 @@ class RaggedPickStream:
                                               self.open.data_ptr(), open_out.data_ptr(), rwork.data_ptr(), rbytes, roff.data_ptr(),
                                               pairs.data_ptr() if pairs.numel() else None, _s()), "seist_ragged_runs_fill")
         self.open = open_out
-        self.look = look_out
+        self.look = st["look_out"]
         self.F = meta["f1"]
         self.closed = last
         return out[0], out[1], (pairs, roff)
@@ -781,6 +796,226 @@ class RaggedStream:
         return RaggedStreamOutput(plan["f0"].tolist(), views, ppk, spk, det)
 
 
+# ---- whole records with data gaps (DESIGN §4.21) ----------------------------------------------------------------------
+_SEG_ROWS = 1 << 16          # segment rows read back by the one host synchronisation of gap_segments
+_MAX_ROWS = 65535            # rows of one ragged pick call (grid.y)
+
+
+class Segments(NamedTuple):
+    """The gap-free segments of a record (S, C, T) (`gap_segments`): a gap sample is one where any channel is not finite,
+    a segment a maximal run of other samples, inclusive [on, off], in station order then time order.  A segment of at
+    least `window` samples is annotated.  On the device: pairs (G, 2) int64 [on, off], offsets (S + 1,) int64 (station s
+    holds segments offsets[s] .. offsets[s + 1] - 1), annotated (G,) bool and station (G,) int64; on the host the planner's
+    copies on, off (G,) and host_offsets (S + 1,) (numpy int64); the (S, T), device and window it was made for."""
+    pairs: torch.Tensor
+    offsets: torch.Tensor
+    annotated: torch.Tensor
+    station: torch.Tensor
+    on: np.ndarray
+    off: np.ndarray
+    host_offsets: np.ndarray
+    shape: Tuple[int, int]
+    device: torch.device
+    window: int
+
+
+def gap_segments(record: torch.Tensor, window: int) -> Segments:
+    """The Segments of record (S, C, T) float32 on a CUDA device for windows of `window` samples.  One pass over the
+    record counts each station's segments, a second writes their [on, off]; one host synchronisation reads the counts and
+    the table (a second one only when the record holds more than 65 536 segments)."""
+    if not record.is_cuda:
+        raise RuntimeError("gap_segments has no CPU path: the record must live on a CUDA device")
+    if record.dtype != torch.float32 or record.dim() != 3:
+        raise ValueError(f"expected a (S, C, T) float32 record, got {tuple(record.shape)} {record.dtype}")
+    S, C, T = record.shape
+    if not (1 <= S <= 65535 and C >= 1 and 1 <= T <= _I32_MAX and int(window) >= 1):
+        raise ValueError(f"need 1 <= S <= 65535, C >= 1, 1 <= T < 2^31 and window >= 1, got {tuple(record.shape)}, window {window}")
+    record = record.contiguous()
+    lib, dev = _lib.lib(), record.device
+    nbytes = lib.seist_runs_work_bytes(S, T)
+    work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    counts = torch.empty(S, dtype=torch.int64, device=dev)
+    _lib.check(lib.seist_gap_segments(record.data_ptr(), S, C, T, work.data_ptr(), nbytes, counts.data_ptr(), _s()), "seist_gap_segments")
+    off = _offsets(counts)
+    cap = min(_SEG_ROWS, S * ((T + 1) // 2))
+    pairs = torch.empty(cap, 2, dtype=torch.int64, device=dev)
+    _lib.check(lib.seist_gap_segments_fill(record.data_ptr(), S, C, T, work.data_ptr(), nbytes, off.data_ptr(), pairs.data_ptr(), cap,
+                                           _s()), "seist_gap_segments_fill")
+    host = torch.cat([off, pairs.view(-1)]).cpu().numpy()                  # the one host synchronisation
+    host_off = host[:S + 1].copy()
+    G = int(host_off[-1])
+    if G > cap:
+        pairs = torch.empty(G, 2, dtype=torch.int64, device=dev)
+        _lib.check(lib.seist_gap_segments_fill(record.data_ptr(), S, C, T, work.data_ptr(), nbytes, off.data_ptr(), pairs.data_ptr(), G,
+                                               _s()), "seist_gap_segments_fill")
+        table = pairs.cpu().numpy().reshape(-1, 2)
+    else:
+        pairs = pairs[:G]
+        table = host[S + 1:S + 1 + 2 * G].reshape(-1, 2)
+    on, off_h = table[:, 0].copy(), table[:, 1].copy()
+    station = torch.repeat_interleave(torch.arange(S, device=dev), counts, output_size=G)     # G is known: no second sync
+    annotated = (pairs[:, 1] - pairs[:, 0] + 1 >= int(window)).contiguous()
+    return Segments(pairs, off, annotated, station, on, off_h, host_off, (S, T), dev, int(window))
+
+
+def check_segments(segs, S: int, T: int, device, window: int | None = None):
+    """Raise ValueError (before any launch) unless segs is a Segments made for a record (S, ., T) on `device` (and for
+    `window` when given), its device tensors of the right dtype, rank and size.  The contents are not read."""
+    if not isinstance(segs, Segments):
+        raise ValueError(f"expected Segments (gap_segments / ContinuousAnnotator.segments), got {type(segs).__name__}")
+    device = torch.device(device)
+    if tuple(segs.shape) != (S, T) or torch.device(segs.device) != device:
+        raise ValueError(f"segments made for (S, T) {tuple(segs.shape)} on {segs.device}, the record is ({S}, {T}) on {device}")
+    if window is not None and segs.window != window:
+        raise ValueError(f"segments made for windows of {segs.window} samples, the annotator's window is {window}")
+    G = len(segs.on)
+    for t, what, dtype, shape in ((segs.pairs, "pairs", torch.int64, (G, 2)), (segs.offsets, "offsets", torch.int64, (S + 1,)),
+                                  (segs.annotated, "annotated", torch.bool, (G,)), (segs.station, "station", torch.int64, (G,))):
+        if not (torch.is_tensor(t) and t.is_cuda and t.device == device and t.dtype == dtype and tuple(t.shape) == shape and
+                t.is_contiguous()):
+            raise ValueError(f"segments.{what}: expected a contiguous {dtype} CUDA tensor of shape {shape} on {device}, "
+                             f"got {tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}"
+                             f"{f' {t.dtype} on {t.device}' if torch.is_tensor(t) else ''}")
+    if len(segs.off) != G or len(segs.host_offsets) != S + 1:
+        raise ValueError(f"segments: host copies of {len(segs.off)} segments and {len(segs.host_offsets)} offsets, expected {G} and {S + 1}")
+
+
+def segment_plan(on, off, window: int, stride: int, batch: int) -> dict:
+    """The packing of all segments' windows, `batch` at a time, from the inclusive [on, off] of each segment (G,): K (G,)
+    = len(window_starts(off - on + 1, window, stride)) for a segment of at least `window` samples, else 0; win_off
+    (G + 1,) its exclusive prefix; first, last (n_batches,) the first and last segment whose windows batch b holds
+    (windows b * batch .. min((b + 1) * batch, win_off[G]) - 1).  numpy int64 arrays."""
+    W, P, B = int(window), int(stride), int(batch)
+    if not (1 <= P <= W and B >= 1):
+        raise ValueError(f"need 1 <= stride <= window and batch >= 1, got stride {P}, window {W}, batch {B}")
+    on = np.asarray(on, dtype=np.int64).reshape(-1)
+    n = np.asarray(off, dtype=np.int64).reshape(-1) - on + 1
+    ann = n >= W
+    kr = np.where(ann, (n - W) // P + 1, 0)
+    K = np.where(ann, kr + ((kr - 1) * P + W < n), 0).astype(np.int64)
+    win_off = _prefix(K)
+    j0 = np.arange(0, int(win_off[-1]), B, dtype=np.int64)
+    j1 = np.minimum(j0 + B, win_off[-1]) - 1
+    first = (np.searchsorted(win_off, j0, "right") - 1).astype(np.int64)
+    last = (np.searchsorted(win_off, j1, "right") - 1).astype(np.int64)
+    return {"K": K, "win_off": win_off, "first": first, "last": last}
+
+
+def segment_window_(x: torch.Tensor, record: torch.Tensor, segs: Segments, win_off: torch.Tensor, n_win: int, window: int, stride: int,
+                    j0: int, norm_mode: str = "std") -> torch.Tensor:
+    """Fill x (B, C, window) in place with the normalised packed segment windows j0 .. j0 + B - 1 (win_off (G + 1,) int64
+    on the device, `segment_plan`), cut from record (S, C, T) in place; ids from n_win on give zero rows."""
+    _dense(record, (None, None, None), "record")
+    S, C, T = record.shape
+    _dense(x, (None, C, window), "window batch", record.device)
+    G = len(segs.on)
+    if n_win > 0 and G:
+        _lib.check(_lib.lib().seist_segment_window(record.data_ptr(), S, C, T, segs.pairs.data_ptr(), segs.station.data_ptr(),
+                                                   win_off.data_ptr(), G, n_win, window, stride, j0, x.shape[0], _MODES[norm_mode],
+                                                   x.data_ptr(), _s()), "seist_segment_window")
+    return x
+
+
+def segment_stack_(probs: torch.Tensor, y: torch.Tensor, segs: Segments, win_off: torch.Tensor, n_win: int, window: int, stride: int,
+                   j0: int, g0: int, g1: int, stack: str = "mean") -> torch.Tensor:
+    """Stack the (B, 3, window) outputs of packed windows j0 .. j0 + B - 1 into probs (S, 3, T) at their segments' samples;
+    g0 .. g1 the segments those windows belong to.  Batches in order from j0 = 0."""
+    _dense(probs, (None, 3, None), "probs")
+    S, _, T = probs.shape
+    _dense(y, (None, 3, window), "window outputs", probs.device)
+    _lib.check(_lib.lib().seist_segment_stack(y.data_ptr(), S, T, segs.pairs.data_ptr(), segs.station.data_ptr(), win_off.data_ptr(),
+                                              len(segs.on), n_win, window, stride, j0, y.shape[0], g0, g1, _STACK[stack],
+                                              probs.data_ptr(), _s()), "seist_segment_stack")
+    return probs
+
+
+def segment_finish_(probs: torch.Tensor, segs: Segments, window: int, stride: int, stack: str = "mean") -> torch.Tensor:
+    """stack="mean": divide every sample of an annotated segment by its covering windows; NaN outside every annotated
+    segment (both modes)."""
+    _dense(probs, (None, 3, None), "probs")
+    S, _, T = probs.shape
+    G = len(segs.on)
+    _lib.check(_lib.lib().seist_segment_finish(probs.data_ptr(), S, T, segs.pairs.data_ptr() if G else None, segs.offsets.data_ptr(),
+                                               G, window, stride, _STACK[stack], _s()), "seist_segment_finish")
+    return probs
+
+
+def segment_groups(lengths, max_rows: int = _MAX_ROWS) -> list:
+    """The picking groups of the annotated segments of lengths (n,): rows whose lengths share a power-of-two class
+    [2^k, 2^(k+1)), in row order, at most max_rows per group.  A group's rows are padded to its longest row, so its
+    work stays within twice its own samples.  A list of int64 row arrays, longest class first."""
+    lengths = np.asarray(lengths, dtype=np.int64).reshape(-1)
+    if lengths.size and lengths.min() < 1:
+        raise ValueError("segment lengths must be positive")
+    cls = np.floor(np.log2(np.maximum(lengths, 1))).astype(np.int64)
+    groups = []
+    for k in np.unique(cls)[::-1]:
+        r = np.nonzero(cls == k)[0].astype(np.int64)
+        groups += [r[i:i + max_rows] for i in range(0, r.size, max_rows)]
+    return groups
+
+
+def pick_segments(probs: torch.Tensor, segs: Segments, thr, mpd: int, det_thr: float = 0.5):
+    """P and S picks (thr = their thresholds) of every annotated segment as its own record, as two per-station CSR
+    (index, prob, offsets) in index order.  The segments are picked as the rows of closing RaggedPickStream calls (row t0
+    = on), one per `segment_groups` group, each group's rows packed by one gather launch; all groups are staged before
+    one host synchronisation reads their totals, and the picks are put back in station and index order on the device."""
+    probs = _check_probs(probs)
+    S, _, T = probs.shape
+    check_segments(segs, S, T, probs.device)
+    if int(mpd) <= 1:
+        raise ValueError(f"min_peak_dist must be > 1 samples, got {mpd}")
+    dev = probs.device
+    length = segs.off - segs.on + 1
+    ann = length >= segs.window
+    rows = np.nonzero(ann)[0].astype(np.int64)                  # row i: the i-th annotated segment
+    m = length[rows]
+    if (m < 3).any():
+        raise ValueError(f"segments of {int(m.min())} samples are too short to pick")
+    if rows.size == 0:
+        return [(torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, device=dev), torch.zeros(S + 1, dtype=torch.int64, device=dev))
+                for _ in range(2)]
+    first_row = _prefix(ann.astype(np.int64))[segs.host_offsets]    # station s's rows start at first_row[s]
+    lib = _lib.lib()
+    staged = []
+    for r in segment_groups(m):
+        n, gm = r.size, m[r]
+        picker = RaggedPickStream(n, dev, mpd, thr[0], thr[1], det_thr, t0=segs.on[rows[r]])
+        host, meta = picker._plan(gm, True)                    # host[:n + 1]: the rows' packed offsets
+        desc = _upload(np.concatenate([rows[r], r, host]), dev)
+        flat = torch.empty(max(1, 3 * int(host[n])), device=dev)
+        _lib.check(lib.seist_segment_gather(probs.data_ptr(), S, T, segs.pairs.data_ptr(), segs.station.data_ptr(), len(segs.on),
+                                            desc.data_ptr(), desc[2 * n:].data_ptr(), n, int(gm.max()), flat.data_ptr(), flat.numel(),
+                                            _s()), "seist_segment_gather")
+        staged.append((picker, desc[n:2 * n], picker._stage(flat, host, desc[2 * n:], meta)))
+    tot = torch.cat([st["totals"] for _, _, st in staged]).tolist()    # the one host synchronisation
+    out = []
+    o = 0
+    picks = []
+    first = _upload(first_row, dev)
+    for picker, _, st in staged:
+        k = st["totals"].numel()
+        picks.append(picker._collect(st, tot[o:o + k], True)[:2])
+        o += k
+    for ch in range(2):
+        counts = torch.zeros(rows.size, dtype=torch.int64, device=dev)   # picks per row, rows in station and index order
+        for (_, pos, _), p in zip(staged, picks):
+            counts.index_copy_(0, pos, p[ch][2][1:] - p[ch][2][:-1])
+        row_off = _offsets(counts)
+        M = sum(p[ch][0].numel() for p in picks)
+        index = torch.empty(M, dtype=torch.int64, device=dev)
+        value = torch.empty(M, dtype=torch.float32, device=dev)
+        for (_, pos, _), p in zip(staged, picks):
+            idx, val, off = p[ch]
+            if idx.numel():
+                row = torch.repeat_interleave(torch.arange(pos.numel(), device=dev), off[1:] - off[:-1], output_size=idx.numel())
+                dest = row_off.index_select(0, pos.index_select(0, row)) + torch.arange(idx.numel(), device=dev) - off.index_select(0, row)
+                index.index_copy_(0, dest, idx)
+                value.index_copy_(0, dest, val)
+        out.append((index, value, row_off.index_select(0, first)))
+    return out
+
+
 class ContinuousAnnotator:
     """`ann = ContinuousAnnotator(model, window=8192, stride=4096, batch=256, norm_mode="std", stack="mean")`
 
@@ -793,6 +1028,9 @@ class ContinuousAnnotator:
       thresholds and min_peak_dist are read here.
     * `st = ann.open_ragged_stream(n_stations)`: the same with stations that advance at different rates
       (`st.push([chunk_s (C, n_s) per station])`, `st.close()`, RaggedStream).
+    * Records with data gaps (non-finite samples): `segs = ann.segments(record)`, then `annotate(record, segments=segs)`
+      and `pick_phases(probs, segments=segs)` treat every gap-free segment of at least `window` samples as a record of
+      its own (NaN elsewhere); `detect_events` needs no segments (DESIGN §4.21).
     Only the seist_*_dpk models (a [det, P, S] probability head) are supported."""
 
     def __init__(self, model, window: int = 8192, stride: int | None = None, batch: int = 256, norm_mode: str = "std",
@@ -832,8 +1070,12 @@ class ContinuousAnnotator:
     def window_count(self, T: int) -> int:
         return len(window_starts(T, self.window, self.stride))
 
+    def segments(self, record: torch.Tensor) -> Segments:
+        """The gap-free segments of record (S, C, T) for this annotator's window (`gap_segments`); one host sync."""
+        return gap_segments(record, self.window)
+
     @torch.no_grad()
-    def annotate(self, record: torch.Tensor) -> torch.Tensor:
+    def annotate(self, record: torch.Tensor, segments: Segments | None = None) -> torch.Tensor:
         dev = next(self.model.parameters()).device
         if not record.is_cuda:
             raise RuntimeError("ContinuousAnnotator has no CPU path: the record must live on the model's CUDA device")
@@ -844,6 +1086,9 @@ class ContinuousAnnotator:
         S, C, T = record.shape
         if C != self.in_channels:
             raise ValueError(f"the model takes {self.in_channels} channels, the record has {C}")
+        if segments is not None:
+            check_segments(segments, S, T, dev, self.window)
+            return self._annotate_segments(record.contiguous(), segments)
         if T < self.window:
             raise ValueError(f"the record ({T} samples) is shorter than one window ({self.window})")
         record = record.contiguous()
@@ -854,6 +1099,22 @@ class ContinuousAnnotator:
             y = self.graph.replay()
             stack_batch_(probs, y, self.window, self.stride, w0, self.stack)
         return stack_finish_(probs, self.window, self.stride, self.stack)
+
+    def _annotate_segments(self, record: torch.Tensor, segs: Segments) -> torch.Tensor:
+        """Every annotated segment as a record of its own, the windows of all segments packed `batch` at a time; NaN
+        outside the annotated segments (DESIGN §4.21)."""
+        S, _, T = record.shape
+        W, P, B = self.window, self.stride, self.batch
+        plan = segment_plan(segs.on, segs.off, W, P, B)
+        n_win = int(plan["win_off"][-1])
+        probs = torch.empty(S, 3, T, dtype=torch.float32, device=record.device)
+        if n_win:
+            win_off = _upload(plan["win_off"], record.device)
+            for b, j0 in enumerate(range(0, n_win, B)):
+                segment_window_(self.graph.x, record, segs, win_off, n_win, W, P, j0, self.norm_mode)
+                y = self.graph.replay()
+                segment_stack_(probs, y, segs, win_off, n_win, W, P, j0, int(plan["first"][b]), int(plan["last"][b]), self.stack)
+        return segment_finish_(probs, segs, W, P, self.stack)
 
     def open_stream(self, n_stations: int) -> ContinuousStream:
         if self.min_peak_dist is None or int(self.min_peak_dist) <= 1:
@@ -867,12 +1128,17 @@ class ContinuousAnnotator:
         return RaggedStream(self, n_stations)
 
     def pick_phases(self, probs: torch.Tensor, ppk_threshold: float | None = None, spk_threshold: float | None = None,
-                    min_peak_dist: int | None = None):
+                    min_peak_dist: int | None = None, segments: Segments | None = None):
         mpd = self.min_peak_dist if min_peak_dist is None else min_peak_dist
         if mpd is None or int(mpd) <= 1:
             raise ValueError(f"min_peak_dist must be > 1 samples, got {mpd}")
         thr = (self.thresholds["ppk"] if ppk_threshold is None else ppk_threshold,
                self.thresholds["spk"] if spk_threshold is None else spk_threshold)
+        if segments is not None:
+            if isinstance(segments, Segments) and segments.window != self.window:
+                raise ValueError(f"segments made for windows of {segments.window} samples, the annotator's window is {self.window}")
+            ppk, spk = pick_segments(probs, segments, thr, int(mpd), self.thresholds["det"])
+            return {"ppk": ppk, "spk": spk}
         ppk, spk = pick_peaks(probs, (1, 2), thr, int(mpd))
         return {"ppk": ppk, "spk": spk}
 
