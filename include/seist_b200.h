@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 18
+#define SEIST_ABI_VERSION 19
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -536,6 +536,31 @@ int seist_segment_gather(const float* probs, int32_t S, int64_t T, const int64_t
 int seist_segment_event_windows(const float* record, int32_t S, int32_t C, int64_t T, const int64_t* pairs, const int64_t* seg_off,
                                 const uint8_t* annotated, int32_t G, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0,
                                 int32_t B, int32_t W, int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream);
+
+/* ---- streams with data gaps (DESIGN §4.22) ----------------------------------------------------------------------------
+   A push of S stations is a packed chunk of chunk_capacity floats: station s's samples are a (C, n_s) block at
+   C * chunk_off[s] (chunk_off (S + 1,) int64, n_s = chunk_off[s + 1] - chunk_off[s] <= max_n); a station whose block does
+   not fit the chunk is read as empty.  Gap samples and segments are those of seist_gap_segments, in each block's own
+   sample index.
+   seist_gap_stream_scan = per station, the number of segments of its block (counts (S,) int64) and, in work
+                           (seist_runs_work_bytes(S, max_n)), per-block offsets for seist_gap_stream_fill, which writes
+                           pairs [on, off] for offsets = the exclusive prefix of counts (rows >= capacity are dropped).
+   seist_gap_stream_pack = out row r (a (C, n_r) block at C * row_off[r], n_r = row_off[r + 1] - row_off[r]) = samples
+                           row_start[r] .. row_start[r] + n_r - 1 of station row_station[r]'s block (0.0f outside it);
+                           n = C * row_off[n_rows] elements, writes past out_capacity are dropped.
+   seist_gap_stream_copy = for every row r, c < 3, t < m_r = m_off[r + 1] - m_off[r]:
+                           dst[dst_base[r] + c * dst_ld[r] + t] = src[src_base[r] + c * src_ld[r] + t]; n = 3 * m_off[n_rows]
+                           elements; reads past src_capacity give NaN, writes past dst_capacity are dropped. */
+int seist_gap_stream_scan(const float* chunk, int64_t chunk_capacity, const int64_t* chunk_off, int32_t S, int32_t C, int64_t max_n,
+                          void* work, int64_t work_bytes, int64_t* counts, void* stream);
+int seist_gap_stream_fill(const float* chunk, int64_t chunk_capacity, const int64_t* chunk_off, int32_t S, int32_t C, int64_t max_n,
+                          const void* work, int64_t work_bytes, const int64_t* offsets, int64_t* pairs, int64_t capacity, void* stream);
+int seist_gap_stream_pack(const float* chunk, int64_t chunk_capacity, const int64_t* chunk_off, int32_t S, int32_t C,
+                          const int64_t* row_station, const int64_t* row_start, const int64_t* row_off, int32_t n_rows, int64_t n,
+                          float* out, int64_t out_capacity, void* stream);
+int seist_gap_stream_copy(const float* src, int64_t src_capacity, const int64_t* m_off, const int64_t* src_base, const int64_t* src_ld,
+                          const int64_t* dst_base, const int64_t* dst_ld, int32_t n_rows, int64_t n, float* dst, int64_t dst_capacity,
+                          void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 18
+ABI_VERSION = 19
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -272,6 +272,14 @@ def lib():
     L.seist_segment_gather.argtypes = [P, I32, I64, P, P, I32, P, P, I32, I64, P, I64, P]
     L.seist_segment_event_windows.restype = C.c_int
     L.seist_segment_event_windows.argtypes = [P, I32, I32, I64, P, P, P, I32, P, I64, P, I64, I32, I32, I32, I32, P, I32, P]
+    L.seist_gap_stream_scan.restype = C.c_int
+    L.seist_gap_stream_scan.argtypes = [P, I64, P, I32, I32, I64, P, I64, P, P]
+    L.seist_gap_stream_fill.restype = C.c_int
+    L.seist_gap_stream_fill.argtypes = [P, I64, P, I32, I32, I64, P, I64, P, P, I64, P]
+    L.seist_gap_stream_pack.restype = C.c_int
+    L.seist_gap_stream_pack.argtypes = [P, I64, P, I32, I32, P, P, P, I32, I64, P, I64, P]
+    L.seist_gap_stream_copy.restype = C.c_int
+    L.seist_gap_stream_copy.argtypes = [P, I64, P, P, P, P, P, I32, I64, P, I64, P]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -312,6 +320,7 @@ EXPORTS = [
     "seist_ragged_history", "seist_ragged_event_windows",
     "seist_gap_segments", "seist_gap_segments_fill", "seist_segment_window", "seist_segment_stack", "seist_segment_finish",
     "seist_segment_gather", "seist_segment_event_windows",
+    "seist_gap_stream_scan", "seist_gap_stream_fill", "seist_gap_stream_pack", "seist_gap_stream_copy",
 ]
 
 

@@ -992,10 +992,8 @@ __device__ __forceinline__ bool gp_ok(const float* x, int C, long long T, long l
   return ok;
 }
 
-// blocks of ST_CH samples; blk (S, nblk): the segment starts of each block
-__global__ void __launch_bounds__(ST_NT) gap_count_kernel(const float* __restrict__ rec, int C, int T, int* __restrict__ blk, int nblk) {
-  __shared__ int warp_s[ST_NT / 32];
-  const float* x = rec + (size_t)blockIdx.y * C * T;
+// the segment starts of block blockIdx.x (ST_CH samples) of the row x (C, T): the CTA's count
+__device__ __forceinline__ int gp_count_block(const float* x, int C, int T, int* warp_s) {
   const int a = blockIdx.x * ST_CH, e = min(a + ST_CH, T), lane = threadIdx.x & 31;
   int n = 0;
   for (int i0 = a; i0 < e; i0 += ST_NT) {
@@ -1005,19 +1003,19 @@ __global__ void __launch_bounds__(ST_NT) gap_count_kernel(const float* __restric
     if (lane == 0) prev = i > 0 && i < e && gp_ok(x, C, T, i - 1);
     n += ok && !prev;
   }
-  n = st_block_count(n, warp_s);
+  return st_block_count(n, warp_s);
+}
+
+// blocks of ST_CH samples; blk (S, nblk): the segment starts of each block
+__global__ void __launch_bounds__(ST_NT) gap_count_kernel(const float* __restrict__ rec, int C, int T, int* __restrict__ blk, int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  const int n = gp_count_block(rec + (size_t)blockIdx.y * C * T, C, T, warp_s);
   if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
 }
 
-// run_fill_kernel with usable / not usable for p > thr: blk holds the exclusive start offsets per block, the ends before a
-// block are as many, less one when a segment crosses into it; rows >= cap are dropped
-__global__ void __launch_bounds__(ST_NT) gap_fill_kernel(const float* __restrict__ rec, int C, int T, const int* __restrict__ blk,
-                                                         int nblk, const long long* __restrict__ offsets, long long cap,
-                                                         long long* __restrict__ pairs) {
-  __shared__ int warp_s[ST_NT / 32];
-  const float* x = rec + (size_t)blockIdx.y * C * T;
+// the [on, off] of the segments of block blockIdx.x of the row x (C, T), the block's first start at table row b0
+__device__ __forceinline__ void gp_fill_block(const float* x, int C, int T, long long b0, long long cap, long long* pairs, int* warp_s) {
   const int a = blockIdx.x * ST_CH, e = min(a + ST_CH, T), lane = threadIdx.x & 31;
-  const long long b0 = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
   long long on_base = b0, off_base = b0 - (a > 0 && gp_ok(x, C, T, a - 1) && gp_ok(x, C, T, a) ? 1 : 0);
   for (int i0 = a; i0 < e; i0 += ST_NT) {
     const int i = i0 + threadIdx.x;
@@ -1033,6 +1031,90 @@ __global__ void __launch_bounds__(ST_NT) gap_fill_kernel(const float* __restrict
     if (foff && off_base + roff >= 0 && off_base + roff < cap) pairs[(off_base + roff) * 2 + 1] = i;
     on_base += ton;
     off_base += toff;
+  }
+}
+
+// run_fill_kernel with usable / not usable for p > thr: blk holds the exclusive start offsets per block, the ends before a
+// block are as many, less one when a segment crosses into it; rows >= cap are dropped
+__global__ void __launch_bounds__(ST_NT) gap_fill_kernel(const float* __restrict__ rec, int C, int T, const int* __restrict__ blk,
+                                                         int nblk, const long long* __restrict__ offsets, long long cap,
+                                                         long long* __restrict__ pairs) {
+  __shared__ int warp_s[ST_NT / 32];
+  const long long b0 = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  gp_fill_block(rec + (size_t)blockIdx.y * C * T, C, T, b0, cap, pairs, warp_s);
+}
+
+// ---- streams with data gaps (DESIGN §4.22) --------------------------------------------------------------------------
+// Station s's pushed samples are a (C, n_s) block at C * chunk_off[s] of a packed chunk of chunk_cap floats; a station
+// whose block does not fit the chunk is read as empty.  The scan is gap_count / gap_fill per block; its table holds
+// each segment's [on, off] in the station's block.
+__device__ __forceinline__ bool gs_block(const long long* chunk_off, long long chunk_cap, int C, int s, long long& b, int& n) {
+  b = chunk_off[s];
+  const long long len = chunk_off[s + 1] - b;
+  n = (int)len;
+  return b >= 0 && len >= 0 && len <= INT32_MAX && C * (b + len) <= chunk_cap;
+}
+
+__global__ void __launch_bounds__(ST_NT) gap_stream_count_kernel(const float* __restrict__ chunk, long long chunk_cap,
+                                                                 const long long* __restrict__ chunk_off, int C, int* __restrict__ blk,
+                                                                 int nblk) {
+  __shared__ int warp_s[ST_NT / 32];
+  long long b;
+  int n;
+  if (!gs_block(chunk_off, chunk_cap, C, blockIdx.y, b, n)) b = n = 0;
+  const int cnt = gp_count_block(chunk + C * b, C, n, warp_s);
+  if (threadIdx.x == 0) blk[(size_t)blockIdx.y * nblk + blockIdx.x] = cnt;
+}
+
+__global__ void __launch_bounds__(ST_NT) gap_stream_fill_kernel(const float* __restrict__ chunk, long long chunk_cap,
+                                                                const long long* __restrict__ chunk_off, int C, const int* __restrict__ blk,
+                                                                int nblk, const long long* __restrict__ offsets, long long cap,
+                                                                long long* __restrict__ pairs) {
+  __shared__ int warp_s[ST_NT / 32];
+  long long b;
+  int n;
+  if (!gs_block(chunk_off, chunk_cap, C, blockIdx.y, b, n) || (long long)blockIdx.x * ST_CH >= n) return;   // uniform per CTA
+  const long long b0 = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
+  gp_fill_block(chunk + C * b, C, n, b0, cap, pairs, warp_s);
+}
+
+// out row r (a (C, n_r) block at C * row_off[r], n_r = row_off[r + 1] - row_off[r]) = samples row_start[r] .. + n_r - 1
+// of station row_station[r]'s block; 0.0f where the row reaches outside that block
+__global__ void __launch_bounds__(ST_NT) gap_stream_pack_kernel(const float* __restrict__ chunk, long long chunk_cap,
+                                                                const long long* __restrict__ chunk_off, int S, int C,
+                                                                const long long* __restrict__ row_station,
+                                                                const long long* __restrict__ row_start,
+                                                                const long long* __restrict__ row_off, int n_rows, long long n,
+                                                                float* __restrict__ out, long long out_cap) {
+  for (long long e = blockIdx.x * (long long)ST_NT + threadIdx.x; e < n && e < out_cap; e += (long long)gridDim.x * ST_NT) {
+    const int r = rg_find((const int64_t*)row_off, n_rows, e / C);
+    const long long m = row_off[r + 1] - row_off[r], i = e - C * row_off[r];
+    float v = 0.f;
+    const long long st = row_station[r];
+    if (m > 0 && i >= 0 && i < C * m && st >= 0 && st < S) {
+      long long b;
+      int ns;
+      const long long c = i / m, t = row_start[r] + (i - c * m);
+      if (gs_block(chunk_off, chunk_cap, C, (int)st, b, ns) && t >= 0 && t < ns) v = chunk[C * b + c * ns + t];
+    }
+    out[e] = v;
+  }
+}
+
+// dst[dst_base[r] + c * dst_ld[r] + t] = src[src_base[r] + c * src_ld[r] + t] for c < 3, t < m_r = m_off[r + 1] - m_off[r];
+// reads past src_cap give NaN, writes past dst_cap are dropped
+__global__ void __launch_bounds__(ST_NT) gap_stream_copy_kernel(const float* __restrict__ src, long long src_cap,
+                                                                const long long* __restrict__ m_off, const long long* __restrict__ src_base,
+                                                                const long long* __restrict__ src_ld, const long long* __restrict__ dst_base,
+                                                                const long long* __restrict__ dst_ld, int n_rows, long long n,
+                                                                float* __restrict__ dst, long long dst_cap) {
+  for (long long e = blockIdx.x * (long long)ST_NT + threadIdx.x; e < n; e += (long long)gridDim.x * ST_NT) {
+    const int r = rg_find((const int64_t*)m_off, n_rows, e / 3);
+    const long long m = m_off[r + 1] - m_off[r], i = e - 3 * m_off[r];
+    if (m <= 0 || i < 0 || i >= 3 * m) continue;
+    const long long c = i / m, t = i - c * m;
+    const long long si = src_base[r] + c * src_ld[r] + t, di = dst_base[r] + c * dst_ld[r] + t;
+    if (di >= 0 && di < dst_cap) dst[di] = si >= 0 && si < src_cap ? src[si] : NAN;
   }
 }
 
@@ -1949,6 +2031,74 @@ int seist_segment_event_windows(const float* record, int32_t S, int32_t C, int64
       M, e0, W, anchor, mode, dst, n_dst);
   note_launch();
   return check_launch("segment_event_windows");
+}
+
+int seist_gap_stream_scan(const float* chunk, int64_t chunk_capacity, const int64_t* chunk_off, int32_t S, int32_t C, int64_t max_n,
+                          void* work, int64_t work_bytes, int64_t* counts, void* stream) {
+  if (!chunk || !chunk_off || !work || !counts || S <= 0 || S > 65535 || C <= 0 || max_n < 1 || max_n > INT32_MAX ||
+      chunk_capacity < 0 || work_bytes < seist_runs_work_bytes(S, max_n)) {
+    set_error("gap_stream_scan: bad arguments (1 <= S <= 65535, C >= 1, 1 <= max_n < 2^31, work >= seist_runs_work_bytes(S, max_n))");
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int* total = (int*)work;
+  int* blk = (int*)((char*)work + st_align(sizeof(int) * S));
+  const int nblk = st_nblk((int)max_n);
+  gap_stream_count_kernel<<<dim3(nblk, S), ST_NT, 0, st>>>(chunk, chunk_capacity, (const long long*)chunk_off, C, blk, nblk);
+  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(blk, nblk, total, (long long*)counts);
+  note_launch();
+  note_launch();
+  return check_launch("gap_stream_scan");
+}
+
+int seist_gap_stream_fill(const float* chunk, int64_t chunk_capacity, const int64_t* chunk_off, int32_t S, int32_t C, int64_t max_n,
+                          const void* work, int64_t work_bytes, const int64_t* offsets, int64_t* pairs, int64_t capacity, void* stream) {
+  if (!chunk || !chunk_off || !work || !offsets || !pairs || S <= 0 || S > 65535 || C <= 0 || max_n < 1 || max_n > INT32_MAX ||
+      chunk_capacity < 0 || capacity < 0 || work_bytes < seist_runs_work_bytes(S, max_n)) {
+    set_error("gap_stream_fill: bad arguments (the work buffer of the seist_gap_stream_scan call, non-null pairs, capacity >= 0)");
+    return -1;
+  }
+  const int* blk = (const int*)((const char*)work + st_align(sizeof(int) * S));
+  const int nblk = st_nblk((int)max_n);
+  gap_stream_fill_kernel<<<dim3(nblk, S), ST_NT, 0, (cudaStream_t)stream>>>(chunk, chunk_capacity, (const long long*)chunk_off, C, blk,
+                                                                            nblk, (const long long*)offsets, capacity, (long long*)pairs);
+  note_launch();
+  return check_launch("gap_stream_fill");
+}
+
+static unsigned gs_grid(long long n) { return (unsigned)std::max<long long>(1, std::min<long long>((n + ST_NT - 1) / ST_NT, 132LL * 16)); }
+
+int seist_gap_stream_pack(const float* chunk, int64_t chunk_capacity, const int64_t* chunk_off, int32_t S, int32_t C,
+                          const int64_t* row_station, const int64_t* row_start, const int64_t* row_off, int32_t n_rows, int64_t n,
+                          float* out, int64_t out_capacity, void* stream) {
+  if (!chunk || !chunk_off || !row_station || !row_start || !row_off || !out || S <= 0 || C <= 0 || n_rows < 1 || n < 0 ||
+      chunk_capacity < 0 || out_capacity < 0) {
+    set_error("gap_stream_pack: bad arguments (non-null buffers and tables, S, C, n_rows >= 1, n >= 0, capacities >= 0)");
+    return -1;
+  }
+  if (n == 0) return 0;
+  gap_stream_pack_kernel<<<gs_grid(n), ST_NT, 0, (cudaStream_t)stream>>>(chunk, chunk_capacity, (const long long*)chunk_off, S, C,
+                                                                         (const long long*)row_station, (const long long*)row_start,
+                                                                         (const long long*)row_off, n_rows, n, out, out_capacity);
+  note_launch();
+  return check_launch("gap_stream_pack");
+}
+
+int seist_gap_stream_copy(const float* src, int64_t src_capacity, const int64_t* m_off, const int64_t* src_base, const int64_t* src_ld,
+                          const int64_t* dst_base, const int64_t* dst_ld, int32_t n_rows, int64_t n, float* dst, int64_t dst_capacity,
+                          void* stream) {
+  if (!src || !m_off || !src_base || !src_ld || !dst_base || !dst_ld || !dst || src == dst || n_rows < 1 || n < 0 || src_capacity < 0 ||
+      dst_capacity < 0) {
+    set_error("gap_stream_copy: bad arguments (non-null, distinct buffers and tables, n_rows >= 1, n >= 0, capacities >= 0)");
+    return -1;
+  }
+  if (n == 0) return 0;
+  gap_stream_copy_kernel<<<gs_grid(n), ST_NT, 0, (cudaStream_t)stream>>>(src, src_capacity, (const long long*)m_off,
+                                                                         (const long long*)src_base, (const long long*)src_ld,
+                                                                         (const long long*)dst_base, (const long long*)dst_ld, n_rows, n,
+                                                                         dst, dst_capacity);
+  note_launch();
+  return check_launch("gap_stream_copy");
 }
 
 }  // extern "C"

@@ -616,10 +616,12 @@ class RaggedPickStream:
         """The per-row descriptor of one call on the host (raises before any launch) and its host-side sizes."""
         S = self.S
         f0, f1 = self.F, self.F + m
-        if last and (f1 - self.t0 < 3).any():
-            short = np.nonzero(f1 - self.t0 < 3)[0]
+        # `last`: one bool for every row, or a per-row bool array (a gapped stream closes some rows only, DESIGN §4.22)
+        last = last if isinstance(last, (bool, np.bool_)) else np.asarray(last, dtype=bool).reshape(S)
+        short = np.nonzero(np.logical_and(last, f1 - self.t0 < 3))[0]
+        if short.size:
             raise ValueError(f"rows {short.tolist()} are too short to pick ({(f1 - self.t0)[short].tolist()} samples)")
-        L = m + 2 + int(last)
+        L = m + 2 + np.asarray(last, dtype=np.int64)
         max_L = int(L.max())
         if max_L > _I32_MAX:
             raise ValueError(f"a stretch of {int(m.max())} samples is too long for one call")
@@ -627,14 +629,14 @@ class RaggedPickStream:
         lo = np.maximum(1, 3 - (f0 - self.t0))
         hi = m.copy()
         rlo = np.full(S, 2, np.int64)
-        rhi = m + 1 + int(last)
+        rhi = m + 1 + np.asarray(last, dtype=np.int64)
         parts = [_prefix(m), _prefix(L), lo, hi, rlo, rhi, g0]
         meta = {"max_L": max_L, "f1": f1, "span": int(max(0, (hi - lo + 1).max())), "rspan": int((rhi - rlo + 1).max()), "ch": {}}
         for ch in (1, 2):
             base = np.minimum(g0, self.first_pend[ch])
             if (f1 - base >= _I32_MAX - 2).any():
                 raise RuntimeError(f"a cluster of candidates spans more than 2^31 samples (channel {ch})")
-            lim = np.full(S, _I64_MAX >> 1, np.int64) if last else f1 - 2 - base
+            lim = np.where(last, _I64_MAX >> 1, f1 - 2 - base).astype(np.int64)
             prev = self.pend[ch]
             delta = base - prev[3] if prev else np.zeros(S, np.int64)
             parts += [lim, base, g0 - base, delta]
@@ -1016,6 +1018,367 @@ def pick_segments(probs: torch.Tensor, segs: Segments, thr, mpd: int, det_thr: f
     return out
 
 
+# ---- streams with data gaps: the segment scan of a push and the host plan of a call (DESIGN §4.22) --------------------
+_GS_ROWS = ("station", "kind", "on", "src", "closes") + _RG_COUNTS
+_CONT, _INTERIOR, _TRAILING = 0, 1, 2
+
+
+def gap_stream_state(n_stations: int) -> dict:
+    """The host state of a fresh gapped stream (`gap_stream_plan`): per station R, the samples pushed; seg_on, the first
+    sample of its open segment (-1: none); seg_R, that segment's samples so far; done, the samples already final."""
+    z = np.zeros(int(n_stations), np.int64)
+    return dict(R=z.copy(), seg_on=np.full(int(n_stations), -1, np.int64), seg_R=z.copy(), done=z.copy())
+
+
+def gap_stream_plan(state: dict, n, pieces, window: int, stride: int, close: bool = False) -> dict:
+    """One call of a gapped stream on the host, from the carried `state` (`gap_stream_state`), the push lengths n (S,)
+    (ignored at the close) and the segments of each station's pushed block, pieces = (station, on, off) (G,) inclusive
+    and in the block's own index, in station then time order.  A row is one station's piece of one segment in this call:
+    kind 0 continues the station's open segment, 1 opens and closes in the push, 2 opens and stays open.  A row closes
+    (`closes`) when a gap sample follows it in the push, or at the close; a closing segment of fewer than `window`
+    samples is no row (its samples come out NaN).  Each row carries ragged_plan's counts f0, r0, f1, r1, k0, nk, tail, kr
+    in its segment's own index, with the close decided per row, and `on` (its segment's first sample in the station's
+    index) and `src` (its first sample in the station's block).  Rows with windows come first, each group in station
+    then time order.  Returns the rows, their win_off, chunk_off, acc_off, out_off (rows + 1,), the stations' output
+    t0 and length m (S,), and the state after the call."""
+    W, P = int(window), int(stride)
+    R, seg_on, seg_R, done = (np.asarray(state[k], dtype=np.int64) for k in ("R", "seg_on", "seg_R", "done"))
+    S = R.size
+    if close:
+        n = np.zeros(S, np.int64)
+        st = a = b = np.zeros(0, np.int64)
+    else:
+        n = np.asarray(n, dtype=np.int64).reshape(-1)
+        if n.shape != R.shape or (n < 0).any():
+            raise ValueError(f"expected {S} non-negative lengths, got {n.tolist()}")
+        st, a, b = (np.asarray(x, dtype=np.int64).reshape(-1) for x in pieces)
+    cont = (a == 0) & (seg_on[st] >= 0)
+    closes = b < n[st] - 1
+    at0 = np.zeros(S, bool)
+    at0[st[a == 0]] = True
+    # an open segment whose push starts with a gap (or the close) ends with no new sample
+    ends = np.nonzero((seg_on >= 0) & (close | ((n > 0) & ~at0)))[0]
+    station = np.concatenate([st, ends])
+    src = np.concatenate([a, np.zeros(ends.size, np.int64)])
+    length = np.concatenate([b - a + 1, np.zeros(ends.size, np.int64)])
+    is_cont = np.concatenate([cont, np.ones(ends.size, bool)])
+    closes = np.concatenate([closes, np.ones(ends.size, bool)])
+    on = np.where(is_cont, seg_on[station], R[station] + src)
+    r0 = np.where(is_cont, seg_R[station], 0)
+    r1 = r0 + length
+    kind = np.where(is_cont, _CONT, np.where(closes, _INTERIOR, _TRAILING))
+    # the state after the call: the open row of each station that pushed, else none
+    new_on, new_R = seg_on.copy(), seg_R.copy()
+    moved = (n > 0) | close
+    new_on[moved], new_R[moved] = -1, 0
+    op = ~closes
+    new_on[station[op]], new_R[station[op]] = on[op], r1[op]
+    R1 = R + n
+    new_done = np.where(new_on >= 0, new_on + np.maximum(new_R - W, 0), R1)
+    keep = op | (r1 >= W)
+    station, src, on, closes, kind, r0, r1 = (x[keep] for x in (station, src, on, closes, kind, r0, r1))
+    f0 = np.maximum(r0 - W, 0)
+    k0 = np.where(r0 >= W, (r0 - W) // P + 1, 0)
+    kr_c = np.where(r1 >= W, (r1 - W) // P + 1, 0)
+    kr = np.where(closes, kr_c, -1)
+    tail = np.where(closes & ((kr_c - 1) * P + W < r1), r1 - W, -1)
+    f1 = np.where(closes, r1, np.maximum(r1 - W, 0))
+    nk = kr_c - k0
+    nw = nk + (tail >= 0)
+    order = np.lexsort((on, station, nw == 0))
+    rows = {k: v[order] for k, v in zip(_GS_ROWS, (station, kind, on, src, closes, f0, r0, f1, r1, k0, nk, tail, kr))}
+    plan = dict(rows)
+    plan["win_off"] = _prefix(nw[order])
+    plan["chunk_off"] = _prefix(rows["r1"] - rows["r0"])
+    plan["acc_off"] = _prefix(rows["r1"] - rows["f0"])
+    plan["out_off"] = _prefix(rows["f1"] - rows["f0"])
+    plan["t0"], plan["m"] = done.copy(), new_done - done
+    plan["state"] = dict(R=R1, seg_on=new_on, seg_R=new_R, done=new_done)
+    return plan
+
+
+def gap_stream_segments(chunk: torch.Tensor, chunk_off, channels: int):
+    """The segments of each station's block of a packed push: station s's samples are a (C, n_s) block at C *
+    chunk_off[s] of chunk (float32 on a CUDA device), chunk_off (S + 1,) on the host.  Returns (station, on, off) (G,)
+    numpy int64, inclusive and in each block's own index, in station then time order: the `pieces` of
+    `gap_stream_plan`.  One host synchronisation reads the counts and a table of at most 65 536 rows (a second one only
+    when the push holds more segments)."""
+    if not chunk.is_cuda:
+        raise RuntimeError("gap_stream_segments has no CPU path: the chunk must live on a CUDA device")
+    chunk_off = np.asarray(chunk_off, dtype=np.int64).reshape(-1)
+    S, C = chunk_off.size - 1, int(channels)
+    n = np.diff(chunk_off)
+    if chunk.dtype != torch.float32 or not chunk.is_contiguous() or S < 1 or S > 65535 or C < 1 or (n < 0).any() or \
+            C * int(chunk_off[-1]) > chunk.numel() or n.max(initial=0) > _I32_MAX:
+        raise ValueError(f"expected a contiguous float32 chunk holding {S} blocks (C, n_s) at C * chunk_off, 1 <= S <= 65535, "
+                         f"0 <= n_s < 2^31, got {tuple(chunk.shape)} {chunk.dtype} and lengths {n.tolist()}")
+    z = np.zeros(0, np.int64)
+    if chunk_off[-1] == 0:
+        return z, z, z
+    lib, dev = _lib.lib(), chunk.device
+    max_n = int(n.max())
+    offs = _upload(chunk_off, dev)
+    nbytes = lib.seist_runs_work_bytes(S, max_n)
+    work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    counts = torch.empty(S, dtype=torch.int64, device=dev)
+    _lib.check(lib.seist_gap_stream_scan(chunk.data_ptr(), chunk.numel(), offs.data_ptr(), S, C, max_n, work.data_ptr(), nbytes,
+                                         counts.data_ptr(), _s()), "seist_gap_stream_scan")
+    off = _offsets(counts)
+    cap = int(min(_SEG_ROWS, ((n + 1) // 2).sum()))
+    pairs = torch.empty(max(cap, 1), 2, dtype=torch.int64, device=dev)
+    _lib.check(lib.seist_gap_stream_fill(chunk.data_ptr(), chunk.numel(), offs.data_ptr(), S, C, max_n, work.data_ptr(), nbytes,
+                                         off.data_ptr(), pairs.data_ptr(), cap, _s()), "seist_gap_stream_fill")
+    host = torch.cat([off, pairs.view(-1)]).cpu().numpy()                  # the one host synchronisation
+    host_off = host[:S + 1]
+    G = int(host_off[-1])
+    if G > cap:
+        pairs = torch.empty(G, 2, dtype=torch.int64, device=dev)
+        _lib.check(lib.seist_gap_stream_fill(chunk.data_ptr(), chunk.numel(), offs.data_ptr(), S, C, max_n, work.data_ptr(), nbytes,
+                                             off.data_ptr(), pairs.data_ptr(), G, _s()), "seist_gap_stream_fill")
+        table = pairs.cpu().numpy().reshape(-1, 2)
+    else:
+        table = host[S + 1:S + 1 + 2 * G].reshape(-1, 2)
+    station = np.repeat(np.arange(S, dtype=np.int64), np.diff(host_off))
+    return station, table[:, 0].copy(), table[:, 1].copy()
+
+
+def _reorder(parts, n_pos: int, first: np.ndarray, dev):
+    """CSR parts [(pos (n,) device int64, values (tuple of (M, ...) tensors), offsets (n + 1,))], row i of a part going to
+    position pos[i] of n_pos -> (values..., offsets at `first` (S + 1,)) with every row's entries at its position, in order."""
+    counts = torch.zeros(n_pos, dtype=torch.int64, device=dev)
+    for pos, _, off in parts:
+        counts.index_copy_(0, pos, off[1:] - off[:-1])
+    row_off = _offsets(counts)
+    out = []
+    for v in range(len(parts[0][1])):
+        M = sum(p[1][v].shape[0] for p in parts)
+        t = parts[0][1][v]
+        dst = torch.empty((M,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+        for pos, vals, off in parts:
+            x = vals[v]
+            if x.shape[0]:
+                row = torch.repeat_interleave(torch.arange(pos.numel(), device=dev), off[1:] - off[:-1], output_size=x.shape[0])
+                dest = row_off.index_select(0, pos.index_select(0, row)) + torch.arange(x.shape[0], device=dev) - off.index_select(0, row)
+                dst.index_copy_(0, dest, x)
+        out.append(dst)
+    return (*out, row_off.index_select(0, _upload(first, dev)))
+
+
+def _copy_rows(src: torch.Tensor, dst: torch.Tensor, m: np.ndarray, src_base, src_ld, dst_base, dst_ld, dev):
+    """seist_gap_stream_copy of the rows with m > 0: (3, m) blocks from src to dst."""
+    sel = np.nonzero(m > 0)[0]
+    if sel.size == 0:
+        return dst
+    m_off = _prefix(m[sel])
+    t = _upload(np.concatenate([m_off] + [np.asarray(x, dtype=np.int64)[sel] for x in (src_base, src_ld, dst_base, dst_ld)]), dev)
+    k = sel.size
+    ptr = [t.data_ptr() + 8 * ((k + 1) + k * i) for i in range(4)]
+    _lib.check(_lib.lib().seist_gap_stream_copy(src.data_ptr(), src.numel(), t.data_ptr(), *ptr, k, 3 * int(m_off[-1]), dst.data_ptr(),
+                                                dst.numel(), _s()), "seist_gap_stream_copy")
+    return dst
+
+
+def _check_chunks(chunks, S: int, C: int, device, what: str):
+    """Raise (before any launch) unless chunks are S contiguous float32 (C, n_s) tensors on `device`."""
+    if len(chunks) != S:
+        raise ValueError(f"expected {S} chunks (one per station), got {len(chunks)}")
+    for s, c in enumerate(chunks):
+        if not torch.is_tensor(c) or not c.is_cuda:
+            raise RuntimeError(f"station {s}: {what} has no CPU path, the chunk must live on the model's CUDA device")
+        if c.device != device:
+            raise RuntimeError(f"station {s}: chunk on {c.device}, model on {device}")
+        if c.dtype != torch.float32 or c.dim() != 2 or c.shape[0] != C:
+            raise ValueError(f"station {s}: expected a ({C}, n) float32 chunk, got {tuple(c.shape)} {c.dtype}")
+        if not c.is_contiguous():
+            raise ValueError(f"station {s}: the chunk must be contiguous")
+
+
+class GapStream:
+    """A stream whose stations' data have gaps (`ContinuousAnnotator.open_gap_stream`): `push(chunks)` and `close()` take
+    what RaggedStream's take and return a RaggedStreamOutput.  A gap sample is one where any channel is not finite, a
+    segment a maximal run of other samples; each segment is streamed as a record of its own, closing in the call that
+    delivers the gap after it.  Per station, concatenated over the calls, probs equal `annotate(rec[None],
+    segments=segments(rec[None]))[0]` of the station's record, the picks `pick_phases` with those segments and the runs
+    `detect_events` (DESIGN §4.22).  Held between calls, per station: the kept raw tail (C, W) and carry (3, W) of its
+    open segment and two picker rows (its open segment's and the next one's)."""
+
+    def __init__(self, ann: "ContinuousAnnotator", n_stations: int):
+        if not 1 <= int(n_stations) <= _MAX_ROWS // 2:
+            raise ValueError(f"need 1 to {_MAX_ROWS // 2} stations (two picker rows each), got {n_stations}")
+        self.ann = ann
+        self.S, self.C = int(n_stations), ann.in_channels
+        self.device = next(ann.model.parameters()).device
+        W = ann.window
+        self.tail = torch.zeros(self.S, self.C, W, device=self.device)
+        self.carry = torch.zeros(self.S, 3, W, device=self.device)
+        self.state = gap_stream_state(self.S)
+        self.flip = np.zeros(self.S, np.int64)          # station s's open segment is picked on row 2s + flip[s]
+        self.forwards = 0
+        self.closed = False
+        thr = ann.thresholds
+        self._thr = (ann.min_peak_dist, thr["ppk"], thr["spk"], thr["det"])
+        self.picker = RaggedPickStream(2 * self.S, self.device, *self._thr)
+        self._none = torch.zeros(1, device=self.device)
+
+    @property
+    def R(self) -> np.ndarray:
+        return self.state["R"]
+
+    @torch.no_grad()
+    def push(self, chunks) -> RaggedStreamOutput:
+        if self.closed:
+            raise RuntimeError("push() after close()")
+        _check_chunks(chunks, self.S, self.C, self.device, "GapStream")
+        n = np.array([c.shape[1] for c in chunks], dtype=np.int64)
+        if n.max(initial=0) > _I32_MAX:
+            raise ValueError(f"a chunk of {int(n.max())} samples is too long for one push")
+        chunk_off = _prefix(n)
+        chunk = torch.cat([c.reshape(-1) for c in chunks]) if chunk_off[-1] else self._none
+        pieces = gap_stream_segments(chunk, chunk_off, self.C)     # the push's first host synchronisation
+        return self._call(gap_stream_plan(self.state, n, pieces, self.ann.window, self.ann.stride), chunk, chunk_off)
+
+    @torch.no_grad()
+    def close(self) -> RaggedStreamOutput:
+        if self.closed:
+            raise RuntimeError("close() after close()")
+        plan = gap_stream_plan(self.state, None, None, self.ann.window, self.ann.stride, close=True)
+        out = self._call(plan, self._none, np.zeros(self.S + 1, np.int64))
+        self.closed = True
+        return out
+
+    def _annotate(self, plan: dict, chunk: torch.Tensor, chunk_off: np.ndarray) -> torch.Tensor:
+        """Every row through the ragged stream's kernels; returns the rows' final probabilities packed at 3 * out_off and
+        writes the station state of every row that stays open."""
+        ann, dev, C, W, P, B = self.ann, self.device, self.C, self.ann.window, self.ann.stride, self.ann.batch
+        lib = _lib.lib()
+        nr = len(plan["station"])
+        probs = torch.empty(max(1, 3 * int(plan["out_off"][-1])), device=dev)
+        if nr == 0:
+            return probs
+        host = np.concatenate([plan[k] for k in _RG_COUNTS + _RG_OFFS] + [plan["station"], plan["src"], plan["closes"].astype(np.int64)])
+        tab = _upload(host, dev)
+        base = tab.data_ptr()
+        cnt = [base + 8 * nr * i for i in range(len(_RG_COUNTS))]
+        o = base + 8 * nr * len(_RG_COUNTS)
+        offp = [o + 8 * (nr + 1) * i for i in range(len(_RG_OFFS))]
+        o += 8 * (nr + 1) * len(_RG_OFFS)
+        t_station = tab[(o - base) // 8:(o - base) // 8 + nr]
+        row_src = o + 8 * nr
+        span = plan["r1"] - plan["f0"]
+
+        def view(ra, rb):
+            return _lib.SeistRaggedStep(*[p + 8 * ra for p in cnt + offp], n_win=int(plan["win_off"][rb]),
+                                        max_len=int(span[ra:rb].max(initial=0)), S=rb - ra, C=C, W=W, P=P,
+                                        norm_mode=_MODES[ann.norm_mode], stack_mode=_STACK[ann.stack])
+
+        # each row's own (C, n_r) block of the push, and the open segment's state for the rows that continue one
+        n_raw = int(plan["chunk_off"][-1])
+        rows_raw = torch.empty(max(1, C * n_raw), device=dev)
+        if n_raw:
+            offs = _upload(chunk_off, dev)
+            _lib.check(lib.seist_gap_stream_pack(chunk.data_ptr(), chunk.numel(), offs.data_ptr(), self.S, C, t_station.data_ptr(), row_src,
+                                                 offp[1], nr, C * n_raw, rows_raw.data_ptr(), rows_raw.numel(), _s()), "seist_gap_stream_pack")
+        tail_in = self.tail.index_select(0, t_station)
+        carry_in = self.carry.index_select(0, t_station)
+        tail_out = torch.empty_like(tail_in)
+        carry_out = torch.empty_like(carry_in)
+        acc = torch.empty(max(1, 3 * int(plan["acc_off"][-1])), device=dev)
+        n_win, woff = int(plan["win_off"][-1]), plan["win_off"]
+        for j0 in range(0, n_win, B):
+            s0 = int(np.searchsorted(woff, j0, "right") - 1)
+            s1 = int(np.searchsorted(woff, min(j0 + B, n_win) - 1, "right") - 1)
+            d = view(s0, s1 + 1)
+            _lib.check(lib.seist_ragged_window(_ref(d), tail_in[s0:].data_ptr(), rows_raw.data_ptr(), j0, B, ann.graph.x.data_ptr(), _s()),
+                       "seist_ragged_window")
+            y = ann.graph.replay()
+            _lib.check(lib.seist_ragged_stack(_ref(d), y.data_ptr(), j0, B, 0, s1 - s0, carry_in[s0:].data_ptr(), acc.data_ptr(), _s()),
+                       "seist_ragged_stack")
+            self.forwards += 1
+        for ra in range(0, nr, _MAX_ROWS):
+            d = view(ra, min(nr, ra + _MAX_ROWS))
+            _lib.check(lib.seist_ragged_emit(_ref(d), carry_in[ra:].data_ptr(), acc.data_ptr(), probs.data_ptr(), carry_out[ra:].data_ptr(),
+                                             _s()), "seist_ragged_emit")
+        op = np.nonzero(~plan["closes"])[0]
+        if op.size:
+            for ra in range(0, nr, _MAX_ROWS // C):
+                d = view(ra, min(nr, ra + _MAX_ROWS // C))
+                _lib.check(lib.seist_ragged_keep(_ref(d), tail_in[ra:].data_ptr(), rows_raw.data_ptr(), tail_out[ra:].data_ptr(), _s()),
+                           "seist_ragged_keep")
+            idx = _upload(np.concatenate([op, plan["station"][op]]), dev)
+            self.tail.index_copy_(0, idx[op.size:], tail_out.index_select(0, idx[:op.size]))
+            self.carry.index_copy_(0, idx[op.size:], carry_out.index_select(0, idx[:op.size]))
+        return probs
+
+    def _call(self, plan: dict, chunk: torch.Tensor, chunk_off: np.ndarray) -> RaggedStreamOutput:
+        S, dev = self.S, self.device
+        rp = self._annotate(plan, chunk, chunk_off)
+        st, kind, m_row = plan["station"], plan["kind"], plan["f1"] - plan["f0"]
+        src_base, out_off = 3 * plan["out_off"][:-1], plan["out_off"]
+        # each station's contiguous output: its rows' final samples, NaN elsewhere
+        m_st, t0 = plan["m"], plan["t0"]
+        st_off = _prefix(m_st)
+        out = torch.full((max(1, 3 * int(st_off[-1])),), float("nan"), device=dev)
+        _copy_rows(rp, out, m_row, src_base, m_row, 3 * st_off[st] + plan["on"] + plan["f0"] - t0[st], m_st[st], dev)
+        # the picker: the open segments' rows of the persistent picker, the interior segments as closing groups
+        pk, flip_old = self.picker, self.flip.copy()
+        cur = 2 * np.arange(S) + flip_old
+        rows_p = np.where(kind == _TRAILING, 2 * st + 1 - flip_old[st], cur[st])
+        trailing = kind == _TRAILING
+        if trailing.any():
+            reset = rows_p[trailing]
+            pk.t0[reset] = pk.F[reset] = plan["on"][trailing]
+            for ch in (1, 2):
+                pk.first_pend[ch][reset] = _I64_MAX
+            r = _upload(reset, dev)
+            pk.look.index_fill_(0, r, float("-inf"))
+            pk.open.index_fill_(0, r, -1)
+            self.flip[st[trailing]] ^= 1
+        pers = kind != _INTERIOR
+        m_p = np.zeros(2 * S, np.int64)
+        last_p = np.zeros(2 * S, bool)
+        m_p[rows_p[pers]] = m_row[pers]
+        last_p[rows_p[pers]] = plan["closes"][pers]
+        pflat = torch.empty(max(1, 3 * int(m_p.sum())), device=dev)
+        p_off = _prefix(m_p)
+        _copy_rows(rp, pflat, m_row[pers], src_base[pers], m_row[pers], 3 * p_off[rows_p[pers]], m_row[pers], dev)
+        # _stage and _collect launch kernels that read the call's descriptor through raw pointers: hold each device copy
+        # here until its _collect has launched
+        host, meta = pk._plan(m_p, last_p)
+        desc = _upload(host, dev)
+        staged = [(pk, desc, pk._stage(pflat, host, desc, meta))]
+        inter = np.nonzero(kind == _INTERIOR)[0]
+        k_st = np.bincount(st[inter], minlength=S).astype(np.int64)
+        base = 2 * np.arange(S, dtype=np.int64) + _prefix(k_st)[:-1]
+        rank = np.arange(inter.size) - np.searchsorted(st[inter], st[inter])     # each interior row's place in its station
+        groups = []
+        for g in segment_groups(m_row[inter]) if inter.size else []:
+            rr = inter[g]
+            gp = RaggedPickStream(rr.size, dev, *self._thr, t0=plan["on"][rr])
+            gh, gm = gp._plan(m_row[rr], True)
+            flat = torch.empty(max(1, 3 * int(gh[rr.size])), device=dev)
+            _copy_rows(rp, flat, m_row[rr], src_base[rr], m_row[rr], 3 * gh[:rr.size], m_row[rr], dev)
+            gd = _upload(gh, dev)
+            staged.append((gp, gd, gp._stage(flat, gh, gd, gm)))
+            groups.append(base[st[rr]] + 1 + rank[g])
+        tot = torch.cat([s["totals"] for _, _, s in staged]).tolist()        # the call's last host synchronisation
+        res, o = [], 0
+        for p, _, s in staged:
+            k = s["totals"].numel()
+            res.append(p._collect(s, tot[o:o + k], False))
+            o += k
+        q = np.arange(2 * S) % 2
+        pos_p = base[np.arange(2 * S) // 2] + np.where(q == flip_old[np.arange(2 * S) // 2], 0, k_st[np.arange(2 * S) // 2] + 1)
+        # per station: its open segment's row, its interior segments in time order, then the row of the segment after them
+        pos = [_upload(x, dev) for x in [pos_p] + groups]
+        n_pos, first = 2 * S + inter.size, np.append(base, 2 * S + inter.size)
+        ppk = _reorder([(ps, r[0][:2], r[0][2]) for ps, r in zip(pos, res)], n_pos, first, dev)
+        spk = _reorder([(ps, r[1][:2], r[1][2]) for ps, r in zip(pos, res)], n_pos, first, dev)
+        det = _reorder([(ps, r[2][:1], r[2][1]) for ps, r in zip(pos, res)], n_pos, first, dev)
+        self.state = plan["state"]
+        views = [out[3 * int(st_off[s]):3 * int(st_off[s + 1])].view(3, int(m_st[s])) for s in range(S)]
+        return RaggedStreamOutput(t0.tolist(), views, ppk, spk, det)
+
+
 class ContinuousAnnotator:
     """`ann = ContinuousAnnotator(model, window=8192, stride=4096, batch=256, norm_mode="std", stack="mean")`
 
@@ -1031,6 +1394,8 @@ class ContinuousAnnotator:
     * Records with data gaps (non-finite samples): `segs = ann.segments(record)`, then `annotate(record, segments=segs)`
       and `pick_phases(probs, segments=segs)` treat every gap-free segment of at least `window` samples as a record of
       its own (NaN elsewhere); `detect_events` needs no segments (DESIGN §4.21).
+    * `st = ann.open_gap_stream(n_stations)`: a ragged stream whose data have gaps, each station's segments streamed as
+      records of their own (`st.push(chunks)`, `st.close()`, GapStream, DESIGN §4.22).
     Only the seist_*_dpk models (a [det, P, S] probability head) are supported."""
 
     def __init__(self, model, window: int = 8192, stride: int | None = None, batch: int = 256, norm_mode: str = "std",
@@ -1126,6 +1491,13 @@ class ContinuousAnnotator:
         if self.min_peak_dist is None or int(self.min_peak_dist) <= 1:
             raise ValueError(f"min_peak_dist must be > 1 samples, got {self.min_peak_dist}")
         return RaggedStream(self, n_stations)
+
+    def open_gap_stream(self, n_stations: int) -> "GapStream":
+        """A ragged stream whose stations' data have gaps (GapStream, at most 32 767 stations); thresholds and
+        min_peak_dist are read here."""
+        if self.min_peak_dist is None or int(self.min_peak_dist) <= 1:
+            raise ValueError(f"min_peak_dist must be > 1 samples, got {self.min_peak_dist}")
+        return GapStream(self, n_stations)
 
     def pick_phases(self, probs: torch.Tensor, ppk_threshold: float | None = None, spk_threshold: float | None = None,
                     min_peak_dist: int | None = None, segments: Segments | None = None):
