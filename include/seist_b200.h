@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 19
+#define SEIST_ABI_VERSION 20
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -488,13 +488,24 @@ int seist_ragged_runs_fill(const float* ext, const int64_t* ext_off, int32_t S, 
    seist_ragged_event_windows = seist_event_windows cutting from a packed history: station s the last one with
                                 offsets[s] <= e (a bounded search), p = index[e] - h0[s] rebased on the device, row s read at
                                 C * hist_off[s] with 0.0f outside [0, len_s) (and past hist_capacity).  Events >= M and
-                                picks outside the station's history give zero rows. */
+                                picks outside the station's history give zero rows.
+   seist_gap_event_windows    = seist_ragged_event_windows for a stream with data gaps (DESIGN §4.23): event e belongs to
+                                position q, the last with pos_off[q] <= e (a bounded search over n_pos + 1 offsets), whose
+                                station pos_station[q] and segment [pos_on[q], pos_end[q]] (global, inclusive) come from the
+                                position table (n_pos entries each); the pick p = index[e] is global.  Samples outside
+                                [on, end] ∩ [h0_s, h0_s + len_s) read as 0.0f (and past hist_capacity), so each window is
+                                that of seist_segment_event_windows on the station's whole record.  Events >= M, a station
+                                outside [0, S) and picks outside that intersection give zero rows. */
 int seist_ragged_history(const float* held, const int64_t* held_off, const int64_t* h0_held, int64_t held_capacity, const float* chunk,
                          const int64_t* chunk_off, int64_t chunk_capacity, const int64_t* h0_out, const int64_t* out_off, int32_t S,
                          int32_t C, int64_t max_len, float* out, int64_t out_capacity, void* stream);
 int seist_ragged_event_windows(const float* hist, const int64_t* hist_off, const int64_t* h0, int64_t hist_capacity, int32_t S,
                                int32_t C, const int64_t* index, int64_t M, const int64_t* offsets, int64_t e0, int32_t B, int32_t W,
                                int32_t anchor, int32_t mode, float* const* x, int32_t n_dst, void* stream);
+int seist_gap_event_windows(const float* hist, const int64_t* hist_off, const int64_t* h0, int64_t hist_capacity, int32_t S, int32_t C,
+                            const int64_t* pos_station, const int64_t* pos_on, const int64_t* pos_end, const int64_t* pos_off,
+                            int32_t n_pos, const int64_t* index, int64_t M, int64_t e0, int32_t B, int32_t W, int32_t anchor, int32_t mode,
+                            float* const* x, int32_t n_dst, void* stream);
 
 /* ---- whole records with data gaps (DESIGN §4.21) ----------------------------------------------------------------------
    Sample t of station s is a gap sample when any channel of record (S, C, T) is not finite; a segment is a maximal run of

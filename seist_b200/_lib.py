@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 19
+ABI_VERSION = 20
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -258,6 +258,8 @@ def lib():
     L.seist_ragged_history.argtypes = [P, P, P, I64, P, P, I64, P, P, I32, I32, I64, P, I64, P]
     L.seist_ragged_event_windows.restype = C.c_int
     L.seist_ragged_event_windows.argtypes = [P, P, P, I64, I32, I32, P, I64, P, I64, I32, I32, I32, I32, P, I32, P]
+    L.seist_gap_event_windows.restype = C.c_int
+    L.seist_gap_event_windows.argtypes = [P, P, P, I64, I32, I32, P, P, P, P, I32, P, I64, I64, I32, I32, I32, I32, P, I32, P]
     L.seist_gap_segments.restype = C.c_int
     L.seist_gap_segments.argtypes = [P, I32, I32, I64, P, I64, P, P]
     L.seist_gap_segments_fill.restype = C.c_int
@@ -321,6 +323,7 @@ EXPORTS = [
     "seist_gap_segments", "seist_gap_segments_fill", "seist_segment_window", "seist_segment_stack", "seist_segment_finish",
     "seist_segment_gather", "seist_segment_event_windows",
     "seist_gap_stream_scan", "seist_gap_stream_fill", "seist_gap_stream_pack", "seist_gap_stream_copy",
+    "seist_gap_event_windows",
 ]
 
 

@@ -793,6 +793,47 @@ __global__ void __launch_bounds__(PR_NT) ragged_event_windows_kernel(const float
       for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = rew_row[i];
 }
 
+// ragged_event_windows_kernel for a gapped stream (DESIGN §4.23): event e is a pick of position q, the last with
+// pos_off[q] <= e (a bounded search, always in [0, n_pos)); the position names its station and its segment's global
+// [on, end].  Samples outside [on, end] ∩ [h0_s, R_s) read as 0.0f, so the window is that of segment_event_windows_kernel.
+// A station outside [0, S), a pick outside its segment or its station's history, and events >= M give zero rows.
+__global__ void __launch_bounds__(PR_NT) gap_event_windows_kernel(const float* __restrict__ hist, const long long* __restrict__ hist_off,
+                                                                  const long long* __restrict__ h0, long long hist_cap, int S, int C,
+                                                                  const long long* __restrict__ pos_station,
+                                                                  const long long* __restrict__ pos_on, const long long* __restrict__ pos_end,
+                                                                  const long long* __restrict__ pos_off, int n_pos,
+                                                                  const long long* __restrict__ index, long long M, long long e0, int W,
+                                                                  int a, int mode, EventDst dst, int n_dst) {
+  extern __shared__ float gew_row[];                // [W]: the zero-filled segment slice of the history, normalised in place
+  const int b = blockIdx.x / C, c = blockIdx.x % C;
+  const long long e = e0 + b;
+  const size_t row = (size_t)blockIdx.x * W;
+  const int q = rg_find((const int64_t*)pos_off, n_pos, e);
+  const long long s = pos_station[q];
+  const bool in = e < M && s >= 0 && s < S;
+  const long long hs = in ? hist_off[s] : 0, len = in ? hist_off[s + 1] - hs : 0, base = in ? h0[s] : 0;
+  const long long lo = max(pos_on[q], base), hi = min(pos_end[q] + 1, base + len);   // readable: [lo, hi), global
+  const long long p = in ? index[e] : -1;
+  if (!in || p < lo || p >= hi) {
+#pragma unroll
+    for (int d = 0; d < EW_MAX_DST; ++d)
+      if (d < n_dst)
+        for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = 0.f;
+    return;
+  }
+  const long long src = C * hs + c * len - base, t0 = p - a;
+  for (int i = threadIdx.x; i < W; i += PR_NT) {
+    const long long t = t0 + i;
+    gew_row[i] = t >= lo && t < hi && src + t >= 0 && src + t < hist_cap ? hist[src + t] : 0.f;
+  }
+  __syncthreads();
+  pr_normalize_row(gew_row, gew_row, W, mode);
+#pragma unroll
+  for (int d = 0; d < EW_MAX_DST; ++d)
+    if (d < n_dst)
+      for (int i = threadIdx.x; i < W; i += PR_NT) dst.x[d][row + i] = gew_row[i];
+}
+
 // channel ch of row s of a packed ext, and its length
 __device__ __forceinline__ const float* rg_row(const float* ext, const long long* __restrict__ ext_off, int C, int ch, int s, long long& L) {
   const long long e0 = ext_off[s];
@@ -1784,6 +1825,33 @@ int seist_ragged_event_windows(const float* hist, const int64_t* hist_off, const
       e0, W, anchor, mode, dst, n_dst);
   note_launch();
   return check_launch("ragged_event_windows");
+}
+
+int seist_gap_event_windows(const float* hist, const int64_t* hist_off, const int64_t* h0, int64_t hist_capacity, int32_t S, int32_t C,
+                            const int64_t* pos_station, const int64_t* pos_on, const int64_t* pos_end, const int64_t* pos_off,
+                            int32_t n_pos, const int64_t* index, int64_t M, int64_t e0, int32_t B, int32_t W, int32_t anchor, int32_t mode,
+                            float* const* x, int32_t n_dst, void* stream) {
+  bool ok = hist && hist_off && h0 && hist_capacity >= 0 && pos_station && pos_on && pos_end && pos_off && n_pos >= 1 &&
+            (index || M == 0) && x && S > 0 && C > 0 && M >= 0 && e0 >= 0 && B > 0 && (long long)B * C <= INT32_MAX && W >= 1 &&
+            W <= 49152 && anchor >= 0 && anchor <= W && mode >= 0 && mode <= 2 && n_dst >= 1 && n_dst <= EW_MAX_DST;
+  EventDst dst{};
+  for (int d = 0; ok && d < n_dst; ++d) ok = (dst.x[d] = x[d]) != nullptr;
+  if (!ok) {
+    set_error("gap_event_windows: bad arguments (non-null history, per-station arrays and position table, n_pos >= 1, "
+              "1 <= W <= 49152, 0 <= anchor <= W, M >= 0, e0 >= 0, B > 0, mode 0 none, 1 std, 2 max, 1 to 4 non-null destinations)");
+    return -1;
+  }
+  static int attr = 0;
+  const int smem = (int)sizeof(float) * W;
+  if (smem > 48 * 1024 && smem > attr) {
+    cudaFuncSetAttribute(gap_event_windows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    attr = smem;
+  }
+  gap_event_windows_kernel<<<(unsigned)((long long)B * C), PR_NT, smem, (cudaStream_t)stream>>>(
+      hist, (const long long*)hist_off, (const long long*)h0, hist_capacity, S, C, (const long long*)pos_station, (const long long*)pos_on,
+      (const long long*)pos_end, (const long long*)pos_off, n_pos, (const long long*)index, M, e0, W, anchor, mode, dst, n_dst);
+  note_launch();
+  return check_launch("gap_event_windows");
 }
 
 int seist_ragged_ext(const float* look, const float* probs, const int64_t* prob_off, const int64_t* ext_off, int32_t S, int32_t C,

@@ -8,7 +8,8 @@ picks of a whole record, as the CSR `ContinuousAnnotator.pick_phases(...)["ppk"]
 static inputs of the models' captured eval plans (`InferenceGraph`) by one kernel launch per batch of events
 (`seist_event_windows`, csrc/stream.cu), and the outputs come back aligned index for index with the pick list.  The numpy
 restatement of the cut is `oracle/event_ref.py`.  `EventCharacterizer.open_stream` does the same for the P picks of a
-record streamed chunk by chunk, in the call that emits them (DESIGN §4.18).  There is no CPU path.
+record streamed chunk by chunk, in the call that emits them (DESIGN §4.18), and `open_ragged_stream` / `open_gap_stream`
+for streams whose stations advance at different rates (§4.20) or whose data have gaps (§4.23).  There is no CPU path.
 """
 from __future__ import annotations
 
@@ -22,6 +23,8 @@ from . import _lib
 from .infer import InferenceGraph
 from .stream import (_I32_MAX, _MODES, ContinuousAnnotator, RaggedStreamOutput, Segments, StreamOutput, _dense, _flat, _prefix, _s,
                      _upload, check_segments)
+
+_HISTORY_ROWS = 65535       # S * C rows of one seist_ragged_history launch (grid.y)
 
 MAX_MODELS = 4              # destinations of one seist_event_windows launch
 MAX_WINDOW = 49152          # a row of the window is staged in shared memory
@@ -191,6 +194,11 @@ class EventCharacterizer:
         """Stations that advance at different rates (`annotator.open_ragged_stream`), every P pick characterised in the call
         that emits it (DESIGN §4.20)."""
         return RaggedCharacterizedStream(self, annotator, n_stations)
+
+    def open_gap_stream(self, annotator: ContinuousAnnotator, n_stations: int) -> "GapCharacterizedStream":
+        """Stations whose data have gaps (`annotator.open_gap_stream`), every P pick characterised in the call that emits
+        it, its window zero outside the pick's own segment (DESIGN §4.23)."""
+        return GapCharacterizedStream(self, annotator, n_stations)
 
 
 def stream_history_(out: torch.Tensor, held: torch.Tensor, h0_held: int, chunk: torch.Tensor | None, h0_out: int) -> torch.Tensor:
@@ -432,3 +440,128 @@ class RaggedCharacterizedStream:
         hist, h0, off = self.buf[0], self.desc[:S], self.desc[S:]
         return RaggedCharacterizedOutput(out, ch._batches(index.numel(), lambda xs, e0: ragged_event_windows_(
             xs, hist, h0, off, index, offsets, e0, ch.window, ch.anchor, ch.norm_mode)))
+
+
+# ---- characterised streams with data gaps (DESIGN §4.23) ----------------------------------------------------------------
+def gap_history_keep(keep, seg_on, R, first_pend, F, anchor: int) -> np.ndarray:
+    """The retention bounds (S,) after one call of a GapCharacterizedStream, from the bounds keep (S,) before it and the
+    state after it: each station's open segment's first sample seg_on (-1 when the station ends the call in a gap), its
+    samples pushed R, and first_pend / F, the first pending P candidate and the final count of its open segment's picker
+    row (station indices).  §4.20's rule on the open segment, clamped at its first sample because no window reads below
+    its own segment: max(keep, seg_on, min(first_pend, F - 1) - anchor); R for a station in a gap, which releases its
+    history at its next non-empty push.  Feeds `ragged_history_plan`."""
+    keep, seg_on, R, first_pend, F = (np.asarray(v, dtype=np.int64).reshape(-1) for v in (keep, seg_on, R, first_pend, F))
+    if not (keep.shape == seg_on.shape == R.shape == first_pend.shape == F.shape):
+        raise ValueError(f"expected (S,) arrays, got {[v.shape for v in (keep, seg_on, R, first_pend, F)]}")
+    k = np.maximum(np.maximum(keep, seg_on), np.minimum(first_pend, F - 1) - int(anchor))
+    return np.where(seg_on >= 0, k, R)
+
+
+def gap_event_windows_(xs, hist: torch.Tensor, hist_h0: torch.Tensor, hist_off: torch.Tensor, pos_station: torch.Tensor,
+                       pos_on: torch.Tensor, pos_end: torch.Tensor, pos_off: torch.Tensor, index: torch.Tensor, e0: int, window: int,
+                       anchor: int, norm_mode: str = "std"):
+    """ragged_event_windows_ for a gapped stream: event e is a pick of position q (the last with pos_off[q] <= e), whose
+    station and global segment [on, end] are pos_station / pos_on / pos_end[q] ((n_pos,) int64 on the device); zeros
+    outside [on, end] ∩ the station's history, so each window equals segment_event_windows_'s on the whole record."""
+    S = hist_h0.numel()
+    dev = hist.device
+    _flat(hist, 0, "histories", dev)
+    _per_station(hist_h0, S, "history h0", dev)
+    _per_station(hist_off, S + 1, "history offsets", dev)
+    n_pos = pos_station.numel()
+    for t, what in ((pos_station, "position stations"), (pos_on, "position segment starts"), (pos_end, "position segment ends")):
+        _per_station(t, n_pos, what, dev)
+    if not 1 <= len(xs) <= MAX_MODELS:
+        raise ValueError(f"1 to {MAX_MODELS} destinations, got {len(xs)}")
+    C = xs[0].shape[1] if xs[0].dim() == 3 else -1
+    for x in xs:
+        _dense(x, (xs[0].shape[0], C, window), "event window batch", dev)
+    _check_picks(index, pos_off, n_pos, dev)
+    if not (1 <= window <= MAX_WINDOW and 0 <= anchor <= window and e0 >= 0 and S >= 1 and 1 <= n_pos <= _I32_MAX):
+        raise ValueError(f"need 1 <= window <= {MAX_WINDOW}, 0 <= anchor <= window, e0 >= 0 and 1 <= n_pos < 2^31, got window "
+                         f"{window}, anchor {anchor}, e0 {e0}, n_pos {n_pos}")
+    ptrs = (ctypes.c_void_p * MAX_MODELS)(*[x.data_ptr() for x in xs])
+    _lib.check(_lib.lib().seist_gap_event_windows(hist.data_ptr(), hist_off.data_ptr(), hist_h0.data_ptr(), hist.numel(), S, C,
+                                                  pos_station.data_ptr(), pos_on.data_ptr(), pos_end.data_ptr(), pos_off.data_ptr(), n_pos,
+                                                  index.data_ptr(), index.numel(), e0, xs[0].shape[0], window, anchor, _MODES[norm_mode],
+                                                  ptrs, len(xs), _s()), "seist_gap_event_windows")
+    return xs
+
+
+class GapCharacterizedStream:
+    """`EventCharacterizer.open_gap_stream(annotator, n_stations)`: `push(chunks)` and `close()` take what `GapStream`'s
+    take (S float32 (C, n_s) tensors, any n_s >= 0, NaN / Inf marking gap samples), each -> RaggedCharacterizedOutput
+    whose `out` is the GapStream's output.  Station s's events, concatenated over the calls, equal `ch(rec_s[None], ppk,
+    segments=segs)` with `segs = annotator.segments(rec_s[None])` and `ppk = annotator.pick_phases(annotator.annotate(
+    rec_s[None], segments=segs), segments=segs)["ppk"]` bit for bit, each in the call that emits its pick (DESIGN §4.23).
+    Each station keeps the raw samples [h0_s, R_s), h0_s the `gap_history_keep` bound of the call before its last
+    non-empty push; the histories are packed as in RaggedCharacterizedStream.  `held_samples` = R - h0 per station ((S,)
+    int64)."""
+
+    def __init__(self, ch: EventCharacterizer, ann: ContinuousAnnotator, n_stations: int):
+        _check_pair(ch, ann)
+        if int(n_stations) * ch.in_channels > _HISTORY_ROWS:
+            raise ValueError(f"{n_stations} stations of {ch.in_channels} channels: the history kernel takes at most "
+                             f"{_HISTORY_ROWS} station channels (S * C)")
+        self.ch = ch
+        self.stream = ann.open_gap_stream(n_stations)
+        self.S, self.C, self.device = self.stream.S, self.stream.C, self.stream.device
+        self.buf = [torch.zeros(1, device=self.device), torch.zeros(1, device=self.device)]
+        self.desc = torch.zeros(2 * self.S + 1, dtype=torch.int64, device=self.device)   # h0 (S,), off (S + 1,) of buf[0]
+        self.h0 = np.zeros(self.S, np.int64)
+        self.R = np.zeros(self.S, np.int64)
+        self.keep = np.zeros(self.S, np.int64)       # the retention bounds after the last call
+
+    @property
+    def closed(self) -> bool:
+        return self.stream.closed
+
+    @property
+    def forwards(self) -> int:
+        return self.stream.forwards
+
+    @property
+    def held_samples(self) -> np.ndarray:
+        return self.R - self.h0
+
+    @torch.no_grad()
+    def push(self, chunks) -> RaggedCharacterizedOutput:
+        n = self.stream._lengths(chunks)                          # validates the chunks before any launch
+        hp = ragged_history_plan(self.h0, self.R, n, self.keep)
+        if (hp["len"] > _I32_MAX).any():
+            s = np.nonzero(hp["len"] > _I32_MAX)[0].tolist()
+            raise ValueError(f"the histories of stations {s} would hold {hp['len'][s].tolist()} samples, more than 2^31 - 1")
+        plan, chunk, chunk_off = self.stream._prepare(chunks)
+        out, where = self.stream._call(plan, chunk, chunk_off)
+        S = self.S
+        hist = [hp["h0"], hp["off"], chunk_off] if n.any() else []
+        dev = _upload(np.concatenate(hist + [where["station"], where["on"], where["end"]]), self.device)   # the call's descriptors
+        if n.any():
+            need = self.C * int(hp["off"][-1])
+            if self.buf[1].numel() < need:
+                self.buf[1] = torch.empty(max(need, 2 * self.buf[1].numel()), device=self.device)
+            ragged_history_(self.buf[1], self.buf[0], self.desc[:S], self.desc[S:], chunk, dev[2 * S + 1:3 * S + 2], dev[:S],
+                            dev[S:2 * S + 1], self.C, int(hp["len"].max()))
+            self.buf.reverse()
+            self.desc = dev[:2 * S + 1]
+            self.h0 = hp["h0"]
+        self.R = hp["R"]
+        return self._finish(out, where, dev[3 * S + 2 if n.any() else 0:])
+
+    @torch.no_grad()
+    def close(self) -> RaggedCharacterizedOutput:
+        out, where = self.stream._close()
+        dev = _upload(np.concatenate([where["station"], where["on"], where["end"]]), self.device)
+        return self._finish(out, where, dev)
+
+    def _finish(self, out: RaggedStreamOutput, where: dict, table: torch.Tensor) -> RaggedCharacterizedOutput:
+        gs, ch, S = self.stream, self.ch, self.S
+        pk, state = gs.picker, gs.state
+        row = 2 * np.arange(S) + gs.flip                       # each station's open-segment row after the call
+        self.keep = gap_history_keep(self.keep, state["seg_on"], state["R"], pk.first_pend[1][row], pk.F[row], ch.anchor)
+        index = out.ppk[0]
+        n_pos = where["station"].size
+        st, on, end = table[:n_pos], table[n_pos:2 * n_pos], table[2 * n_pos:3 * n_pos]
+        hist, h0, off, pos_off = self.buf[0], self.desc[:S], self.desc[S:], where["pos_off"]
+        return RaggedCharacterizedOutput(out, ch._batches(index.numel(), lambda xs, e0: gap_event_windows_(
+            xs, hist, h0, off, st, on, end, pos_off, index, e0, ch.window, ch.anchor, ch.norm_mode)))

@@ -1144,7 +1144,8 @@ def gap_stream_segments(chunk: torch.Tensor, chunk_off, channels: int):
 
 def _reorder(parts, n_pos: int, first: np.ndarray, dev):
     """CSR parts [(pos (n,) device int64, values (tuple of (M, ...) tensors), offsets (n + 1,))], row i of a part going to
-    position pos[i] of n_pos -> (values..., offsets at `first` (S + 1,)) with every row's entries at its position, in order."""
+    position pos[i] of n_pos -> ((values..., offsets at `first` (S + 1,)), the offsets of every position (n_pos + 1,))
+    with every row's entries at its position, in order."""
     counts = torch.zeros(n_pos, dtype=torch.int64, device=dev)
     for pos, _, off in parts:
         counts.index_copy_(0, pos, off[1:] - off[:-1])
@@ -1161,7 +1162,37 @@ def _reorder(parts, n_pos: int, first: np.ndarray, dev):
                 dest = row_off.index_select(0, pos.index_select(0, row)) + torch.arange(x.shape[0], device=dev) - off.index_select(0, row)
                 dst.index_copy_(0, dest, x)
         out.append(dst)
-    return (*out, row_off.index_select(0, _upload(first, dev)))
+    return (*out, row_off.index_select(0, _upload(first, dev))), row_off
+
+
+def gap_pick_positions(plan: dict, flip) -> dict:
+    """Where the picks of one gapped-stream call go, from its `gap_stream_plan` and each station's open-row flip before
+    the call (GapStream: station s's open segment is picked on row 2s + flip[s]).  Station s owns positions first[s] ..
+    first[s + 1] - 1: its open segment's picker row, its k_s interior segments in time order, then the picker row of the
+    segment after them.  Returns rows_p (rows,): each row's persistent picker row (the open one for interior rows);
+    pos_p (2S,): each persistent picker row's position; inter: the interior rows and pos_i their positions; n_pos and
+    first (S + 1,); and the position table station, on, end (n_pos,) int64: the segment [on, end] (station index,
+    inclusive) whose picks land at each position.  end is on + r1 - 1 for a row that closes and R - 1 after the call
+    for one that stays open; a position without a row in the call emits no pick and gets [0, -1] (DESIGN §4.23)."""
+    flip = np.asarray(flip, dtype=np.int64).reshape(-1)
+    S = flip.size
+    st, kind = plan["station"], plan["kind"]
+    rows_p = np.where(kind == _TRAILING, 2 * st + 1 - flip[st], 2 * st + flip[st])
+    inter = np.nonzero(kind == _INTERIOR)[0]
+    k_st = np.bincount(st[inter], minlength=S).astype(np.int64)
+    base = 2 * np.arange(S, dtype=np.int64) + _prefix(k_st)[:-1]
+    rank = np.arange(inter.size) - np.searchsorted(st[inter], st[inter])     # each interior row's place in its station
+    s_p = np.arange(2 * S) // 2
+    pos_p = base[s_p] + np.where(np.arange(2 * S) % 2 == flip[s_p], 0, k_st[s_p] + 1)
+    pos_i = base[st[inter]] + 1 + rank
+    n_pos = 2 * S + inter.size
+    row_pos = pos_p[rows_p]
+    row_pos[inter] = pos_i
+    on, end = np.zeros(n_pos, np.int64), np.full(n_pos, -1, np.int64)
+    on[row_pos] = plan["on"]
+    end[row_pos] = np.where(plan["closes"], plan["on"] + plan["r1"] - 1, plan["state"]["R"][st] - 1)
+    return dict(rows_p=rows_p, pos_p=pos_p, inter=inter, pos_i=pos_i, n_pos=n_pos, first=np.append(base, n_pos),
+                station=np.repeat(np.arange(S, dtype=np.int64), k_st + 2), on=on, end=end)
 
 
 def _copy_rows(src: torch.Tensor, dst: torch.Tensor, m: np.ndarray, src_base, src_ld, dst_base, dst_ld, dev):
@@ -1226,25 +1257,37 @@ class GapStream:
 
     @torch.no_grad()
     def push(self, chunks) -> RaggedStreamOutput:
+        return self._call(*self._prepare(chunks))[0]
+
+    def _lengths(self, chunks) -> np.ndarray:
+        """Validate a push (raises before any launch) -> its lengths n (S,)."""
         if self.closed:
             raise RuntimeError("push() after close()")
         _check_chunks(chunks, self.S, self.C, self.device, "GapStream")
         n = np.array([c.shape[1] for c in chunks], dtype=np.int64)
         if n.max(initial=0) > _I32_MAX:
             raise ValueError(f"a chunk of {int(n.max())} samples is too long for one push")
+        return n
+
+    def _prepare(self, chunks):
+        """Validate, pack and scan a push -> (the call's plan, the chunks packed at C * chunk_off[s], chunk_off)."""
+        n = self._lengths(chunks)
         chunk_off = _prefix(n)
         chunk = torch.cat([c.reshape(-1) for c in chunks]) if chunk_off[-1] else self._none
         pieces = gap_stream_segments(chunk, chunk_off, self.C)     # the push's first host synchronisation
-        return self._call(gap_stream_plan(self.state, n, pieces, self.ann.window, self.ann.stride), chunk, chunk_off)
+        return gap_stream_plan(self.state, n, pieces, self.ann.window, self.ann.stride), chunk, chunk_off
 
     @torch.no_grad()
     def close(self) -> RaggedStreamOutput:
+        return self._close()[0]
+
+    def _close(self):
         if self.closed:
             raise RuntimeError("close() after close()")
         plan = gap_stream_plan(self.state, None, None, self.ann.window, self.ann.stride, close=True)
-        out = self._call(plan, self._none, np.zeros(self.S + 1, np.int64))
+        res = self._call(plan, self._none, np.zeros(self.S + 1, np.int64))
         self.closed = True
-        return out
+        return res
 
     def _annotate(self, plan: dict, chunk: torch.Tensor, chunk_off: np.ndarray) -> torch.Tensor:
         """Every row through the ragged stream's kernels; returns the rows' final probabilities packed at 3 * out_off and
@@ -1309,7 +1352,9 @@ class GapStream:
             self.carry.index_copy_(0, idx[op.size:], carry_out.index_select(0, idx[:op.size]))
         return probs
 
-    def _call(self, plan: dict, chunk: torch.Tensor, chunk_off: np.ndarray) -> RaggedStreamOutput:
+    def _call(self, plan: dict, chunk: torch.Tensor, chunk_off: np.ndarray):
+        """One call -> (its RaggedStreamOutput, where its P picks came from: `gap_pick_positions`' table station, on, end
+        (host) and pos_off, the device offsets (n_pos + 1,) of the P picks by position)."""
         S, dev = self.S, self.device
         rp = self._annotate(plan, chunk, chunk_off)
         st, kind, m_row = plan["station"], plan["kind"], plan["f1"] - plan["f0"]
@@ -1320,9 +1365,9 @@ class GapStream:
         out = torch.full((max(1, 3 * int(st_off[-1])),), float("nan"), device=dev)
         _copy_rows(rp, out, m_row, src_base, m_row, 3 * st_off[st] + plan["on"] + plan["f0"] - t0[st], m_st[st], dev)
         # the picker: the open segments' rows of the persistent picker, the interior segments as closing groups
-        pk, flip_old = self.picker, self.flip.copy()
-        cur = 2 * np.arange(S) + flip_old
-        rows_p = np.where(kind == _TRAILING, 2 * st + 1 - flip_old[st], cur[st])
+        pk = self.picker
+        where = gap_pick_positions(plan, self.flip)
+        rows_p = where["rows_p"]
         trailing = kind == _TRAILING
         if trailing.any():
             reset = rows_p[trailing]
@@ -1346,10 +1391,7 @@ class GapStream:
         host, meta = pk._plan(m_p, last_p)
         desc = _upload(host, dev)
         staged = [(pk, desc, pk._stage(pflat, host, desc, meta))]
-        inter = np.nonzero(kind == _INTERIOR)[0]
-        k_st = np.bincount(st[inter], minlength=S).astype(np.int64)
-        base = 2 * np.arange(S, dtype=np.int64) + _prefix(k_st)[:-1]
-        rank = np.arange(inter.size) - np.searchsorted(st[inter], st[inter])     # each interior row's place in its station
+        inter = where["inter"]
         groups = []
         for g in segment_groups(m_row[inter]) if inter.size else []:
             rr = inter[g]
@@ -1359,24 +1401,23 @@ class GapStream:
             _copy_rows(rp, flat, m_row[rr], src_base[rr], m_row[rr], 3 * gh[:rr.size], m_row[rr], dev)
             gd = _upload(gh, dev)
             staged.append((gp, gd, gp._stage(flat, gh, gd, gm)))
-            groups.append(base[st[rr]] + 1 + rank[g])
+            groups.append(where["pos_i"][g])
         tot = torch.cat([s["totals"] for _, _, s in staged]).tolist()        # the call's last host synchronisation
         res, o = [], 0
         for p, _, s in staged:
             k = s["totals"].numel()
             res.append(p._collect(s, tot[o:o + k], False))
             o += k
-        q = np.arange(2 * S) % 2
-        pos_p = base[np.arange(2 * S) // 2] + np.where(q == flip_old[np.arange(2 * S) // 2], 0, k_st[np.arange(2 * S) // 2] + 1)
         # per station: its open segment's row, its interior segments in time order, then the row of the segment after them
-        pos = [_upload(x, dev) for x in [pos_p] + groups]
-        n_pos, first = 2 * S + inter.size, np.append(base, 2 * S + inter.size)
-        ppk = _reorder([(ps, r[0][:2], r[0][2]) for ps, r in zip(pos, res)], n_pos, first, dev)
-        spk = _reorder([(ps, r[1][:2], r[1][2]) for ps, r in zip(pos, res)], n_pos, first, dev)
-        det = _reorder([(ps, r[2][:1], r[2][1]) for ps, r in zip(pos, res)], n_pos, first, dev)
+        pos = [_upload(x, dev) for x in [where["pos_p"]] + groups]
+        n_pos, first = where["n_pos"], where["first"]
+        ppk, pos_off = _reorder([(ps, r[0][:2], r[0][2]) for ps, r in zip(pos, res)], n_pos, first, dev)
+        spk, _ = _reorder([(ps, r[1][:2], r[1][2]) for ps, r in zip(pos, res)], n_pos, first, dev)
+        det, _ = _reorder([(ps, r[2][:1], r[2][1]) for ps, r in zip(pos, res)], n_pos, first, dev)
         self.state = plan["state"]
         views = [out[3 * int(st_off[s]):3 * int(st_off[s + 1])].view(3, int(m_st[s])) for s in range(S)]
-        return RaggedStreamOutput(t0.tolist(), views, ppk, spk, det)
+        table = {k: where[k] for k in ("station", "on", "end")}
+        return RaggedStreamOutput(t0.tolist(), views, ppk, spk, det), dict(table, pos_off=pos_off)
 
 
 class ContinuousAnnotator:
