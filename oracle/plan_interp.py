@@ -46,11 +46,62 @@ def rng_u16(step_seed: int, stream: int, idx: np.ndarray) -> np.ndarray:
     return ((h >> (np.uint64(16) * (idx & np.uint64(3)))) & np.uint64(0xFFFF)).astype(np.uint32)
 
 
+def _drop_threshold(p: float) -> int:
+    """csrc/common.cuh::drop_threshold: round(p * 65536) in fp32, at most 65535."""
+    return int(min(np.rint(np.float32(p) * np.float32(65536.0)), np.float32(65535.0)))
+
+
 def keep_mask(p: float, step_seed: int, stream: int, idx: np.ndarray) -> torch.Tensor:
     """1/(1-p) where kept, 0 where dropped (drop probability quantised to 2^-16 like the CUDA side)."""
-    thr = np.uint32(min(np.rint(np.float32(p) * np.float32(65536.0)), np.float32(65535.0)))
-    keep = rng_u16(step_seed, stream, idx) >= thr
+    keep = rng_u16(step_seed, stream, idx) >= np.uint32(_drop_threshold(p))
     return torch.from_numpy(keep.astype(np.float32)) / np.float32(1.0 - np.float32(p))
+
+
+# ---- the same generator on torch int64 tensors, for masks built on the interpreter's device ------------------------
+# torch has no uint64 arithmetic: the hash runs on int64 with the same bits.  Multiplies wrap modulo 2^64 like the
+# unsigned ones, the right shifts are arithmetic and are made logical by masking the sign-extended high bits, and the
+# Python-int constants are reduced to their two's complement int64 value.
+def _i64(v: int) -> int:
+    v &= M64
+    return v - (1 << 64) if v >> 63 else v
+
+
+def _srl(z: torch.Tensor, s: int) -> torch.Tensor:
+    return (z >> s) & ((1 << (64 - s)) - 1)
+
+
+def rng_u64_t(step_seed: int, stream: int, qidx: torch.Tensor) -> torch.Tensor:
+    """rng_u64 on an int64 tensor of quad indices; the uint64 result as int64 bits."""
+    z = qidx.to(torch.int64) * _i64(0x9E3779B97F4A7C15)
+    z += _i64(step_seed * 0xD1342543DE82EF95 + ((stream << 32) | 0x9E3779B9))
+    z ^= _srl(z, 30)
+    z *= _i64(0xBF58476D1CE4E5B9)
+    z ^= _srl(z, 27)
+    z *= _i64(0x94D049BB133111EB)
+    z ^= _srl(z, 31)
+    return z
+
+
+def rng_u16_t(step_seed: int, stream: int, idx: torch.Tensor) -> torch.Tensor:
+    """rng_u16 on an int64 tensor of element indices."""
+    idx = idx.to(torch.int64)
+    return (rng_u64_t(step_seed, stream, _srl(idx, 2)) >> ((idx & 3) * 16)) & 0xFFFF
+
+
+def keep_mask_t(p: float, step_seed: int, stream: int, idx: torch.Tensor) -> torch.Tensor:
+    """keep_mask on an int64 tensor of element indices, on that tensor's device."""
+    keep = rng_u16_t(step_seed, stream, idx) >= _drop_threshold(p)
+    return keep.to(torch.float32) / np.float32(1.0 - np.float32(p))
+
+
+def keep_mask_range(p: float, step_seed: int, stream: int, n: int, device) -> torch.Tensor:
+    """keep_mask of the element indices 0 .. n-1, built on `device`: one hash per quad, its four 16-bit lanes in
+    order, so a mask of N*C*L elements costs N*C*L/4 hashes and no index array of its own size."""
+    h = rng_u64_t(step_seed, stream, torch.arange((n + 3) // 4, dtype=torch.int64, device=device))
+    thr = _drop_threshold(p)
+    keep = torch.stack([(_srl(h, 16 * j) & 0xFFFF) >= thr for j in range(4)], 1).view(-1)[:n]
+    del h
+    return keep.to(torch.float32) / np.float32(1.0 - np.float32(p))
 
 
 def upsample_linear(X: torch.Tensor, size: int) -> torch.Tensor:
@@ -179,19 +230,25 @@ class Interp:
         X = F.pad(X, (f.pad_left, pr))
         return F.conv1d(X, W, None, stride=f.stride, groups=f.groups)
 
+    def _mask(self, p: float, stream: int, n: int) -> torch.Tensor:
+        """keep_mask of the element indices 0 .. n-1 in the interpreter's dtype, on its device: built there for a CUDA
+        plan (a mask of a full-length layer at a production batch is 10^8 elements), with numpy for a CPU plan."""
+        seed = int(self.p.step_seed.item())
+        if self.dev.type == "cuda":
+            return keep_mask_range(p, seed, stream, n, self.dev).to(self.dt)
+        return keep_mask(p, seed, stream, np.arange(n, dtype=np.uint64)).to(self.dev, self.dt)
+
     def _drop_factor(self, f: Op):
         """delta(n) * D(n,c,l) multiplying conv+bias, and alpha(n)."""
         N, C, L = f.N, f.Cout, f.L_out
-        seed = int(self.p.step_seed.item())
         fac = torch.ones(N, C, L, dtype=self.dt, device=self.dev)
         if f.p_elem > 0:
-            idx = np.arange(N * C * L, dtype=np.uint64)
-            fac = fac * keep_mask(f.p_elem, seed, f.seed_elem, idx).view(N, C, L).to(self.dev, self.dt)
+            fac = fac * self._mask(f.p_elem, f.seed_elem, N * C * L).view(N, C, L)
         if f.p_path > 0:
-            fac = fac * keep_mask(f.p_path, seed, f.seed_path, np.arange(N, dtype=np.uint64)).view(N, 1, 1).to(self.dev, self.dt)
+            fac = fac * self._mask(f.p_path, f.seed_path, N).view(N, 1, 1)
         alpha = torch.ones(N, 1, 1, dtype=self.dt, device=self.dev)
         if f.p_alpha > 0:
-            alpha = keep_mask(f.p_alpha, seed, f.seed_alpha, np.arange(N, dtype=np.uint64)).view(N, 1, 1).to(self.dev, self.dt)
+            alpha = self._mask(f.p_alpha, f.seed_alpha, N).view(N, 1, 1)
         return fac, alpha
 
     def _W(self, f: Op):
@@ -241,8 +298,7 @@ class Interp:
         lse = torch.logsumexp(s, -1)
         if f.p_attn > 0:
             Lk = kh.shape[-1]
-            idx = np.arange(N * H * Lq * Lk, dtype=np.uint64)
-            a = a * keep_mask(f.p_attn, int(self.p.step_seed.item()), f.seed_attn, idx).view(N, H, Lq, Lk).to(self.dev, self.dt)
+            a = a * self._mask(f.p_attn, f.seed_attn, N * H * Lq * Lk).view(N, H, Lq, Lk)
         o = (a @ vh.transpose(-1, -2)).transpose(-1, -2).reshape(N, C, Lq)
         return o, lse
 

@@ -13,6 +13,12 @@ from seist_b200.models import create_model
 ZERO_DROPS = dict(path_drop_rate=0, attn_drop_rate=0, key_drop_rate=0, mlp_drop_rate=0, other_drop_rate=0)
 
 
+def model_drops(name):
+    """The drop rates model `name` trains with when nobody sets them (its registered preset), as a `drops` dict."""
+    hp = create_model(name, in_channels=3, in_samples=8192).hp
+    return {k: getattr(hp, k) for k in ZERO_DROPS}
+
+
 def randomize(model, seed=0, wstd=0.25):
     """Non-degenerate parameters / running statistics (random-init eval output is a flat 0.5, SURVEY §0.6)."""
     g = torch.Generator().manual_seed(seed)

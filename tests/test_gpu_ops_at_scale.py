@@ -18,7 +18,8 @@ Two criteria per checked quantity:
 
 The three GPU tests take about 90 s together on an H100 (two ~11 GB arenas, float64 reference on the device).
 test_gpu_ops_at_scale_variants.py runs the same check (`check_at_scale(name, n, length, training)`) on the other
-production configurations: a ragged input length, the s and l model sizes and the vector heads.
+production configurations: a ragged input length, the s and l model sizes and the vector heads;
+test_gpu_ops_at_scale_dropout.py runs it with the model's default drop rates, as the benchmark trains.
 """
 import ctypes
 import gc
@@ -133,13 +134,13 @@ def _per_cta(tiles, waves, gy_gz, sm=SM_COUNT):
     return tiles / gx
 
 
-def loop_counts(name, n, length, training=True, tcc_all=False):
+def loop_counts(name, n, length, training=True, tcc_all=False, drops=None):
     """Per persistent family, one (phase, op index, row length, count) per op: quads per pw_fwd thread, tiles per
     tcconv CTA (the default dispatch rule, or every eligible op with `tcc_all`, as SEIST_TCC=1), strided chunks per
     bwwk CTA and per bww CTA (1x1 and the k-tap convs that bwwk has no kernel for) - from the plan's op fields only
-    (no CUDA library)."""
+    (no CUDA library).  `drops`: the drop rates of the plan (None: no dropout)."""
     m = create_model(name, in_channels=3, in_samples=length)
-    m.set_drop_rates(**ZERO_DROPS)
+    m.set_drop_rates(**(ZERO_DROPS if drops is None else drops))
     pl = P.PlanBuilder(m, P.FlatState(m, torch.device("cpu")), n, length, training).build()
     out = {what: [] for what in LOOP_FAMILY}
     for i, f in enumerate(pl.fwd_ops):
@@ -309,6 +310,10 @@ class _Report:
         self.chan_failures = []     # per-channel criterion
         self.worst = {}             # (family, quantity) -> (ratio, where)
         self.pool_ties = 0          # max-pool windows left out of the data-gradient comparison
+        self.op = None              # (phase, op index) being checked
+        self.drop = ""              # its dropout variant (drop_label)
+        self.checked = set()        # (phase, op index) of every op held to the per-channel criterion
+        self.sites = set()          # dropout_sites of the plan
 
     def whole(self, where, what, got, ref):
         err, mx = rel_err(got, ref)
@@ -316,12 +321,16 @@ class _Report:
             self.failures.append(f"{where} {what}: rel {err:.3e} (max {mx:.3e})")
 
     def chan(self, family, where, what, got, ref, scale, dim=1, mask=None, partial_tile=False):
-        """`partial_tile`: a tcconv op whose rows end in a partial 128-sample tile, also reported on its own line."""
+        """`partial_tile`: a tcconv op whose rows end in a partial 128-sample tile, also reported on its own line; an op
+        that applies a dropout mask or factor is also reported under its family with the variant appended."""
         if mask is not None:
             got, ref, scale, dim = got[mask], ref[mask], scale[mask], 0
         r, c = chan_err(got, ref, scale, dim)
+        self.checked.add(self.op)
         key = (family, what)
-        for k in [key, (family + " partial tile", what)] if partial_tile else [key]:
+        keys = [key] + ([(family + " partial tile", what)] if partial_tile else []) + \
+            ([(f"{family} {self.drop}", what)] if self.drop else [])
+        for k in keys:
             if k not in self.worst or r > self.worst[k][0]:
                 self.worst[k] = (r, f"{where} channel {c}")
         tol = CHAN_TOL.get(key)
@@ -333,6 +342,25 @@ def _families(c_ops):
     lib = _lib.lib()
     base, size = ctypes.addressof(c_ops), ctypes.sizeof(_lib.SeistOp)
     return [lib.seist_op_family(base + i * size).decode() for i in range(len(c_ops))]
+
+
+def drop_label(kind, f):
+    """The dropout an op of `kind` applies, its forward op `f` holding the rates: "p_elem" (element mask of a conv
+    output, with its per-sample factors), "p_path" (per-sample stochastic-depth factors only), "p_alpha" (the
+    residual's factor that RES_BWD applies), "p_attn" (attention-weight mask), or ""."""
+    if kind in (_lib.CONV_FWD, _lib.CONV_BWD_DATA, _lib.CONV_BWD_W):
+        return "p_elem" if f.p_elem > 0 else ("p_path" if f.p_path > 0 or f.p_alpha > 0 else "")
+    if kind == _lib.RES_BWD:
+        return "p_alpha" if f.p_alpha > 0 else ""
+    if kind in (_lib.ATT_FWD, _lib.ATT_BWD_Q, _lib.ATT_BWD_KV):
+        return "p_attn" if f.p_attn > 0 else ""
+    return ""
+
+
+def dropout_sites(pl):
+    """{(phase, op index)} of every op whose kernel applies a dropout mask or factor."""
+    return {("fwd", i) for i, f in enumerate(pl.fwd_ops) if drop_label(f.kind, f)} | \
+        {("bwd", i) for i, op in enumerate(pl.bwd_ops) if op.fwd is not None and drop_label(op.kind, op.fwd)}
 
 
 def _stat_slices(p, v):
@@ -358,19 +386,23 @@ def _calibrated_state(name, length, steps=40):
     return {k: v.detach().cpu() for k, v in m.state_dict().items()}
 
 
-def run_at_scale(name, n, length, training):
-    """Runs every op of the plan on the kernels and on the float64 interpreter; returns the _Report."""
+def run_at_scale(name, n, length, training, drops=None, step_seed=12345):
+    """Runs every op of the plan on the kernels and on the float64 interpreter; returns the _Report.  `drops`: the
+    drop rates (None: no dropout); `step_seed`: the dropout step counter, an unsigned 64-bit value."""
     sd = None if training else _calibrated_state(name, length)
-    p_ref, p_gpu, it, _, _ = build_pair(name, n, length, training, ref_device="cuda", ref_dtype=D, state_dict=sd)
+    p_ref, p_gpu, it, _, _ = build_pair(name, n, length, training, drops=drops, ref_device="cuda", ref_dtype=D,
+                                        state_dict=sd)
     rep = _Report()
+    rep.sites = dropout_sites(p_ref)
     g = torch.Generator().manual_seed(1)
-    p_ref.step_seed.fill_(12345)
+    p_ref.step_seed.fill_(step_seed - (1 << 64) if step_seed >> 63 else step_seed)     # int64 holds the same bits
     p_ref.x_in.x.copy_(torch.randn(n, 3, length, generator=g))
     p_ref.stat.zero_()
 
     for i, (fr, fg, fam) in enumerate(zip(p_ref.fwd_ops, p_gpu.fwd_ops, _families(p_gpu.c_fwd))):
         push_state(p_ref, p_gpu)
         where = f"fwd[{i}] {fr.name}"
+        rep.op, rep.drop = ("fwd", i), drop_label(fr.kind, fr)
         mag = None
         pt = fam.startswith("tcconv") and fr.L_out % 128 != 0
         if fr.kind == _lib.CONV_FWD:
@@ -419,6 +451,7 @@ def run_at_scale(name, n, length, training):
             run_gpu_op(p_gpu, p_gpu.c_bwd, i - 1)
         where = f"bwd[{i}] {br.name}"
         f = br.fwd
+        rep.op, rep.drop = ("bwd", i), (drop_label(br.kind, f) if f is not None else "")
         pt = fam.startswith("tcconv") and f.L_in % 128 != 0
         # deposits checked against a magnitude: (ref target, gpu target, elementwise magnitude or None = max-abs)
         deposits = []
@@ -492,31 +525,35 @@ def _release():
     torch.cuda.empty_cache()
 
 
-def check_at_scale(name, n, length, training):
+def check_at_scale(name, n, length, training, drops=None, step_seed=12345):
     """run_at_scale on one configuration; prints the worst per-channel ratio of every (family, quantity) it reached and
-    fails on any whole-tensor or per-channel failure."""
+    fails on any whole-tensor or per-channel failure, or on a dropout site that was not held to the per-channel
+    criterion."""
     t0 = time.time()
     try:
-        rep = run_at_scale(name, n, length, training)
+        rep = run_at_scale(name, n, length, training, drops, step_seed)
     finally:
         _release()
-    print(f"\n{name} N={n} L={length} training={training} SEIST_TCC={os.environ.get('SEIST_TCC', '')}: "
-          f"{time.time() - t0:.0f} s; {rep.pool_ties} max-pool near ties left out; "
-          "worst per-channel error / magnitude by family:")
+    print(f"\n{name} N={n} L={length} training={training} SEIST_TCC={os.environ.get('SEIST_TCC', '')}"
+          + (f" drops={drops} step_seed={step_seed}" if drops is not None else "") +
+          f": {time.time() - t0:.0f} s; {rep.pool_ties} max-pool near ties left out; "
+          + (f"{len(rep.sites)} dropout sites; " if rep.sites else "") + "worst per-channel error / magnitude by family:")
     for (fam, what), (r, where) in sorted(rep.worst.items()):
         print(f"  {fam:40s} {what:6s} {r:.3e}  ({where})")
-    failures = rep.failures[:20] + rep.chan_failures[:20]
-    assert not failures, f"{len(rep.failures)} + {len(rep.chan_failures)} failures:\n" + "\n".join(failures)
+    unchecked = [f"{ph}[{i}]: dropout site not checked" for ph, i in sorted(rep.sites - rep.checked)]
+    failures = rep.failures[:20] + rep.chan_failures[:20] + unchecked[:20]
+    assert not failures, f"{len(rep.failures)} + {len(rep.chan_failures)} + {len(unchecked)} failures:\n" + \
+        "\n".join(failures)
     return rep
 
 
-def check_on_tensor_cores(name, n, length, families=("tcconv_bwd",)):
+def check_on_tensor_cores(name, n, length, families=("tcconv_bwd",), drops=None, step_seed=12345):
     """check_at_scale in a child process with SEIST_TCC=1 (read once per process): every eligible forward /
     data-gradient conv runs on the persistent wgmma engine.  Each of `families` must prefix a family that ran."""
     _release()
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     code = ("import sys; sys.path.insert(0, 'tests'); import test_gpu_ops_at_scale as T;"
-            f"rep = T.check_at_scale({name!r}, {n}, {length}, True);"
+            f"rep = T.check_at_scale({name!r}, {n}, {length}, True, {drops!r}, {step_seed});"
             f"missing = [p for p in {tuple(families)!r} if not any(f.startswith(p) for f, _ in rep.worst)];"
             "assert not missing, ('no op of these families ran', missing);"
             "print('TC-OK')")
