@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 20
+#define SEIST_ABI_VERSION 21
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -572,6 +572,28 @@ int seist_gap_stream_pack(const float* chunk, int64_t chunk_capacity, const int6
 int seist_gap_stream_copy(const float* src, int64_t src_capacity, const int64_t* m_off, const int64_t* src_base, const int64_t* src_ld,
                           const int64_t* dst_base, const int64_t* dst_ld, int32_t n_rows, int64_t n, float* dst, int64_t dst_capacity,
                           void* stream);
+
+/* ---- polyphase resampling (DESIGN §4.24) -------------------------------------------------------------------------------
+   scipy.signal.resample_poly(x, up, down, axis=-1) with its defaults (window ('kaiser', 5.0), zeros outside the record) for
+   1 <= up, down <= 256 (the ratio reduced by the caller): output k of a row of T inputs, k < ceil(T * up / down), lies at input time k * down / up and is
+   the fp32 fmaf chain over the in-record inputs i in ascending order of x[i] * h[k * down - i * up + hl], where the tap index
+   lies in [0, 2 * hl] and hl = 10 * max(up, down).  Out-of-record inputs are skipped, not multiplied by zero, so an output is
+   NaN exactly when a NaN input lies in its support.  taps: up phases of nt = 2 * hl / up + 1 floats each, phase phi holding
+   h[phi + (nt_phi - 1 - t) * up] at taps[phi * nt + t] for t < nt_phi = (2 * hl - phi) / up + 1 (the order of ascending i).
+   Every output of every call is computed by one device function, so a stream's outputs are bit-identical to the record's.
+   seist_resample        = record (rows, T) -> out (rows, ceil(T * up / down)), one launch.
+   seist_resample_stream = one call of S stations of C channels: desc is a device int64 array of N0, lo0, K0, lo1 (S each) then
+                           chunk_off and out_off (S + 1 each).  Station s has received N0[s] inputs, holds inputs lo0 ..
+                           N0 - 1 at held row (s, c) (held (S, C, H)), and has emitted outputs 0 .. K0 - 1; the push brings
+                           n_s = chunk_off[s + 1] - chunk_off[s] inputs as a (C, n_s) block at C * chunk_off[s] of chunk.  The
+                           call writes outputs K0 .. K0 + m_s - 1 (m_s = out_off[s + 1] - out_off[s]) as a (C, m_s) block at
+                           C * out_off[s] of out, and inputs lo1 .. N0 + n_s - 1 to held_out row (s, c) (distinct from held).
+                           Those outputs must have all their in-record inputs among lo0 .. N0 + n_s - 1; max_m >= every m_s sizes
+                           the grid.  One launch; a malformed descriptor gives wrong output but no out-of-range access. */
+int seist_resample(const float* record, int32_t rows, int64_t T, const float* taps, int32_t up, int32_t down, float* out, void* stream);
+int seist_resample_stream(const float* held, int64_t H, const float* chunk, int64_t chunk_capacity, const int64_t* desc, int32_t S,
+                          int32_t C, int64_t max_m, const float* taps, int32_t up, int32_t down, float* out, int64_t out_capacity,
+                          float* held_out, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);
