@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 21
+#define SEIST_ABI_VERSION 22
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -231,6 +231,15 @@ int seist_huber_bwd(const float* preds, const float* targets, const float* gout,
 int seist_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t numel,
                     const float* lr, const float* step, double beta1, double beta2, double eps,
                     double weight_decay, int32_t decoupled, float grad_scale, void* stream);
+/* torch.optim.SGD(momentum, dampening, weight_decay, nesterov) single fused update over one flat buffer —
+   training/train.py:316-322.  d = grad_scale * g (+ weight_decay * p); with momentum != 0 the buffer is d on the
+   first step and momentum * buf + (1 - dampening) * d after it, and d becomes buf (or d + momentum * buf with
+   nesterov); p -= lr * d.  The first step is *step <= 1 on the device (the caller increments step before the call),
+   so the call is graph-replayable.  momentum_buf may be NULL when momentum == 0; nesterov needs momentum > 0 and
+   dampening == 0. */
+int seist_sgd_step(float* params, const float* grads, float* momentum_buf, int64_t numel, const float* lr,
+                   const float* step, double momentum, double dampening, double weight_decay, int32_t nesterov,
+                   float grad_scale, void* stream);
 
 /* Gradient all-reduce (sum) over peer memory: out[i] = sum_p grad_peer[p][i], bracketed by two cross-rank
    barriers (all gradients complete / all peers finished reading).  `comm` is the DEVICE copy; graph capturable. */

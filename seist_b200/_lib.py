@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 21
+ABI_VERSION = 22
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -153,6 +153,9 @@ def lib():
     L.seist_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                   C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int32,
                                   C.c_float, C.c_void_p]
+    L.seist_sgd_step.restype = C.c_int
+    L.seist_sgd_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_double,
+                                 C.c_double, C.c_double, C.c_int32, C.c_float, C.c_void_p]
     L.seist_advance_seed.restype = C.c_int
     L.seist_advance_seed.argtypes = [C.c_void_p, C.c_void_p]
     L.seist_pick_phase.restype = C.c_int
@@ -312,7 +315,7 @@ def lib():
 EXPORTS = [
     "seist_abi_version", "seist_sizeof_op", "seist_sizeof_bn", "seist_last_error", "seist_launch_count",
     "seist_tc_error_flag", "seist_plan_run", "seist_plan_run_lanes", "seist_bce_fwd", "seist_bce_bwd", "seist_huber_fwd", "seist_huber_bwd",
-    "seist_adam_step", "seist_advance_seed", "seist_comm_allreduce", "seist_comm_barrier", "seist_sizeof_comm", "seist_op_family",
+    "seist_adam_step", "seist_sgd_step", "seist_advance_seed", "seist_comm_allreduce", "seist_comm_barrier", "seist_sizeof_comm", "seist_op_family",
     "seist_pick_phase", "seist_detect_event", "seist_pick_counters", "seist_det_counters",
     "seist_normalize", "seist_dpk_labels", "seist_ce_fwd", "seist_ce_bwd",
     "seist_augment", "seist_sizeof_aug", "seist_aug_recipe_bytes",

@@ -1,4 +1,4 @@
-// Small kernels: regression/classification head, BatchNorm finalisation, fused losses, fused Adam.
+// Small kernels: regression/classification head, BatchNorm finalisation, fused losses, fused Adam and SGD.
 #include "common.cuh"
 
 namespace seist {
@@ -375,6 +375,32 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
   }
 }
 
+// ================================================================================================
+// SGD
+// ================================================================================================
+// torch.optim.SGD's arithmetic: momentum and weight decay are cast to fp32 as torch does with python floats, (1 - dampening)
+// is formed in double first.  The first step (buf = d, no dampening) is read from the device step counter, so a
+// captured launch replays correctly after the eager warm-up step: step <= 1 means "no buffer yet".
+__global__ void __launch_bounds__(256) sgd_kernel(float* __restrict__ p, const float* __restrict__ g,
+                                                  float* __restrict__ buf, int64_t n, const float* __restrict__ lr_p,
+                                                  const float* __restrict__ step_p, double momd, double dampd,
+                                                  double wdd, int nesterov, float gscale) {
+  const float lr = *lr_p;
+  const bool first = *step_p <= 1.f;
+  const float mom = (float)momd, omd = (float)(1.0 - dampd), wd = (float)wdd;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float pi = p[i];
+    float d = g[i] * gscale;
+    if (wdd != 0.0) d = fmaf(wd, pi, d);
+    if (momd != 0.0) {
+      const float b = first ? d : fmaf(omd, d, mom * buf[i]);
+      buf[i] = b;
+      d = nesterov ? fmaf(mom, b, d) : b;
+    }
+    p[i] = fmaf(-lr, d, pi);
+  }
+}
+
 __global__ void advance_seed_kernel(uint64_t* s) { *s += 1; }
 
 }  // namespace seist
@@ -459,6 +485,22 @@ int seist_adam_step(float* params, const float* grads, float* exp_avg, float* ex
                                              weight_decay, decoupled, grad_scale);
   note_launch();
   return check_launch("adam_step");
+}
+
+int seist_sgd_step(float* params, const float* grads, float* momentum_buf, int64_t numel, const float* lr,
+                   const float* step, double momentum, double dampening, double weight_decay, int32_t nesterov,
+                   float grad_scale, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (numel <= 0) return -1;
+  if (momentum != 0.0 && momentum_buf == nullptr) { set_error("sgd_step: momentum needs a momentum buffer"); return -2; }
+  if (nesterov && (momentum <= 0.0 || dampening != 0.0)) {
+    set_error("sgd_step: nesterov needs a positive momentum and zero dampening");
+    return -2;
+  }
+  sgd_kernel<<<ew_grid(numel), 256, 0, s>>>(params, grads, momentum_buf, numel, lr, step, momentum, dampening,
+                                            weight_decay, nesterov, grad_scale);
+  note_launch();
+  return check_launch("sgd_step");
 }
 
 int seist_advance_seed(uint64_t* seed, void* stream) {
