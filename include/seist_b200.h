@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 22
+#define SEIST_ABI_VERSION 23
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -368,20 +368,7 @@ int seist_event_windows(const float* record, int32_t S, int32_t C, int64_t T, co
                          window ran in an earlier call starts from carry.  Call with j0 = 0, B, 2B, ... in order.
    seist_stream_emit   = probs (mean: one IEEE division by the number of covering windows; max as is) and carry_out.
    seist_stream_keep   = tail_out.
-   Picking a stream takes the final probabilities in stretches.  ext (S, C, L) holds, per row, the two samples before the
-   stretch, the stretch and at the close one -inf sentinel; ext sample i is global sample g0 + i.
-   seist_stream_peaks  = the rising-edge candidates of ext[s, channel] at i in [lo, hi] go behind the ones still pending
-                         from the previous call's work `prev` (prev_capc, prev_L; null on the first call), rebased by
-                         -delta; candidates are held as int32 offsets from `base` (candidate i: i + ishift).  Clusters
-                         (gaps <= mpd) whose last candidate c has c + mpd <= lim are resolved as in seist_peaks_long; the
-                         rest stay pending.  counts (S,) int64: picks; info (2S,) int64: pending count, global index of the
-                         first pending candidate (INT64_MAX when none).  work: seist_stream_peaks_work_bytes(S, capc, L);
-                         capc >= max pending + L / 2 + 1.  seist_stream_peaks_fill writes the picks (global index = base +
-                         offset) as seist_peaks_long_fill does.
-   seist_stream_runs   = the runs of ext[s, channel] > threshold that end in this stretch: position p in [lo, hi] closes a
-                         run at p - 1 or opens one at p.  open_in (S,) int64: the start of the run open before the stretch
-                         (-1: none); open_out: the same after it.  counts (S,) int64; work: seist_runs_work_bytes(S, L).
-                         seist_stream_runs_fill writes the [on, off] pairs (global) at pairs[offsets[s] ..]. */
+   The final probabilities are picked by seist_ragged_peaks and seist_ragged_runs, every row a stretch of f1 - f0. */
 typedef struct SeistStreamStep {
   int64_t f0, r0, f1, r1;
   int64_t k0;          /* first regular window of the call */
@@ -402,26 +389,6 @@ int seist_stream_stack(const SeistStreamStep* step, const float* y, int64_t j0, 
 int seist_stream_emit(const SeistStreamStep* step, const float* carry, const float* acc, float* probs, float* carry_out,
                       void* stream);
 int seist_stream_keep(const SeistStreamStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream);
-/* Raw history of a characterised stream (DESIGN §4.18): held (S, C, n_held) holds the global samples
-   [h0_held, h0_held + n_held) of every row, chunk (S, C, n) the n samples after them.  out (S, C, n_out) = the samples
-   [h0_out, h0_held + n_held + n), n_out = h0_held + n_held + n - h0_out, rows packed at stride n_out; out_capacity (floats)
-   >= S * C * n_out and out overlaps neither input.  Needs 0 <= h0_held <= h0_out, 0 <= n_out < 2^31, S * C <= 65535; each
-   retained sample is read and written once, and n_out = 0 launches nothing (out may then be null).  seist_event_windows cuts from out with
-   T = n_out and the pick indices rebased by -h0_out. */
-int seist_stream_history(const float* held, int64_t h0_held, int64_t n_held, const float* chunk, int64_t n, int64_t h0_out,
-                         int32_t S, int32_t C, float* out, int64_t out_capacity, void* stream);
-int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L);
-int seist_stream_peaks(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float mph,
-                       int32_t min_peak_dist, int64_t lim, int64_t base, int32_t ishift, void* work, int32_t capc,
-                       const void* prev, int32_t prev_capc, int64_t prev_L, int64_t delta, int32_t max_pend, int64_t* counts,
-                       int64_t* info, void* stream);
-int seist_stream_peaks_fill(int32_t S, int64_t L, const void* work, int32_t capc, int64_t base, const int64_t* offsets,
-                            int64_t* index, float* value, void* stream);
-int seist_stream_runs(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float threshold,
-                      const int64_t* open_in, int64_t* open_out, void* work, int64_t work_bytes, int64_t* counts, void* stream);
-int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi,
-                           float threshold, int64_t g0, const int64_t* open_in, int64_t* open_out, const void* work,
-                           int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream);
 
 /* ---- ragged streams: stations that advance at different rates (DESIGN §4.19) -----------------------------------------
    One call of a ragged stream is SeistStreamStep per station: every per-station count is a device int64 array of S
@@ -444,12 +411,22 @@ int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t chann
    seist_ragged_ext    = ext from look (S, C, 2) and the stretches (probs packed at C * prob_off[s], (C, m_s)), every
                          sample past them -inf (the sentinel when L_s = m_s + 3), plus look_out (S, C, 2) = ext samples
                          m_s, m_s + 1 of each row.
-   seist_ragged_peaks  = seist_stream_peaks with lo, hi, lim, base, ishift (= g0 - base) and delta per row (device int64
-                         arrays); lo is raised to 1 and hi lowered to L_s - 2 in the kernels.  max_span >= max(hi - lo + 1)
-                         and max_L = max L_s size the grids; work: seist_stream_peaks_work_bytes(S, capc, max_L).
-                         seist_ragged_peaks_fill writes the picks (global index = base[s] + offset).
-   seist_ragged_runs   = seist_stream_runs with lo, hi and g0 per row (hi lowered to L_s - 1); work:
-                         seist_runs_work_bytes(S, max_L). */
+   ext sample i of row s is global sample g0[s] + i.  lo, hi, lim, base, ishift, delta and g0 are per-row device int64
+   arrays; max_span >= max(hi - lo + 1) and max_L = max L_s size the grids.
+   seist_ragged_peaks  = the rising-edge candidates of ext[s, channel] at i in [max(lo, 1), min(hi, L_s - 2)] go behind the
+                         ones still pending from the previous call's work `prev` (prev_capc, prev_L; null on the first
+                         call), rebased by -delta[s]; candidates are held as int32 offsets from base[s] (candidate i:
+                         i + ishift[s], ishift = g0 - base).  Clusters (gaps <= mpd) whose last candidate c has
+                         c + mpd <= lim[s] are resolved as in seist_peaks_long; the rest stay pending.  counts (S,) int64:
+                         picks; info (2S,) int64: pending count, global index of the first pending candidate (INT64_MAX
+                         when none).  work: seist_stream_peaks_work_bytes(S, capc, max_L); capc >= max pending +
+                         max_L / 2 + 1.  seist_ragged_peaks_fill writes the picks (global index = base[s] + offset) as
+                         seist_peaks_long_fill does.
+   seist_ragged_runs   = the runs of ext[s, channel] > threshold that end in this stretch: position p in
+                         [max(lo, 1), min(hi, L_s - 1)] closes a run at p - 1 or opens one at p.  open_in (S,) int64: the
+                         start of the run open before the stretch (-1: none); open_out: the same after it.  counts (S,)
+                         int64; work: seist_runs_work_bytes(S, max_L).  seist_ragged_runs_fill writes the [on, off] pairs
+                         (global) at pairs[offsets[s] ..]. */
 typedef struct SeistRaggedStep {
   const int64_t *f0, *r0, *f1, *r1, *k0, *nk, *tail, *kr;   /* (S,) each */
   const int64_t *win_off, *chunk_off, *acc_off, *out_off;    /* (S + 1,) each */
@@ -470,6 +447,7 @@ int seist_ragged_emit(const SeistRaggedStep* step, const float* carry, const flo
 int seist_ragged_keep(const SeistRaggedStep* step, const float* tail_raw, const float* chunk, float* tail_out, void* stream);
 int seist_ragged_ext(const float* look, const float* probs, const int64_t* prob_off, const int64_t* ext_off, int32_t S, int32_t C,
                      int64_t max_L, float* ext, float* look_out, void* stream);
+int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L);
 int seist_ragged_peaks(const float* ext, const int64_t* ext_off, int32_t S, int32_t C, int32_t channel, int64_t max_L,
                        const int64_t* lo, const int64_t* hi, int64_t max_span, float mph, int32_t min_peak_dist,
                        const int64_t* lim, const int64_t* base, const int64_t* ishift, void* work, int32_t capc,
@@ -485,14 +463,15 @@ int seist_ragged_runs_fill(const float* ext, const int64_t* ext_off, int32_t S, 
                            const int64_t* open_in, int64_t* open_out, const void* work, int64_t work_bytes,
                            const int64_t* offsets, int64_t* pairs, void* stream);
 
-/* ---- raw histories of a ragged characterised stream (DESIGN §4.20) ---------------------------------------------------
+/* ---- raw histories of characterised streams (DESIGN §4.18, §4.20) ----------------------------------------------------
    A packed history holds station s as a (C, len_s) block at C * off[s], len_s = off[s + 1] - off[s], whose first sample
    is the station's global sample h0[s]; off (S + 1,) and h0 (S,) are device int64 arrays, never read back to the host.
-   seist_ragged_history       = the packed counterpart of seist_stream_history: out row (s, c) = the samples
+   seist_ragged_history       = the raw history of a characterised stream after a push: out row (s, c) = the samples
                                 [h0_out[s], h0_out[s] + len_out_s) of the held row (held_off, h0_held) followed by the
-                                station's block of the chunk packed as in SeistRaggedStep (chunk_off).  max_len >= every
-                                len_out_s sizes the grid (0 launches nothing); reads outside a station's own held and chunk
-                                blocks or past a buffer's capacity (floats) give 0.0f, writes past out_capacity are dropped.
+                                station's block of the chunk packed as in SeistRaggedStep (chunk_off); each retained sample
+                                is read and written once.  max_len >= every len_out_s sizes the grid (0 launches nothing);
+                                reads outside a station's own held and chunk blocks or past a buffer's capacity (floats)
+                                give 0.0f, writes past out_capacity are dropped.
                                 out overlaps neither input; S * C <= 65535.
    seist_ragged_event_windows = seist_event_windows cutting from a packed history: station s the last one with
                                 offsets[s] <= e (a bounded search), p = index[e] - h0[s] rebased on the device, row s read at

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 22
+ABI_VERSION = 23
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -217,25 +217,8 @@ def lib():
     L.seist_stream_emit.argtypes = [step, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.seist_stream_keep.restype = C.c_int
     L.seist_stream_keep.argtypes = [step, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.seist_stream_history.restype = C.c_int
-    L.seist_stream_history.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
-                                       C.c_void_p, C.c_int64, C.c_void_p]
     L.seist_stream_peaks_work_bytes.restype = C.c_int64
     L.seist_stream_peaks_work_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int64]
-    L.seist_stream_peaks.restype = C.c_int
-    L.seist_stream_peaks.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
-                                     C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
-                                     C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.seist_stream_peaks_fill.restype = C.c_int
-    L.seist_stream_peaks_fill.argtypes = [C.c_int32, C.c_int64, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_void_p]
-    L.seist_stream_runs.restype = C.c_int
-    L.seist_stream_runs.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
-                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
-    L.seist_stream_runs_fill.restype = C.c_int
-    L.seist_stream_runs_fill.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_float,
-                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                         C.c_void_p]
     rstep = C.POINTER(SeistRaggedStep)
     P, I32, I64, F32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     L.seist_sizeof_ragged_step.restype = C.c_uint64
@@ -322,8 +305,7 @@ EXPORTS = [
     "seist_window_batch", "seist_event_windows", "seist_stack_batch", "seist_stack_finish", "seist_peaks_work_bytes", "seist_peaks_long",
     "seist_peaks_long_fill", "seist_runs_work_bytes", "seist_runs_long", "seist_runs_long_fill",
     "seist_sizeof_stream_step", "seist_stream_window", "seist_stream_stack", "seist_stream_emit", "seist_stream_keep",
-    "seist_stream_history",
-    "seist_stream_peaks_work_bytes", "seist_stream_peaks", "seist_stream_peaks_fill", "seist_stream_runs", "seist_stream_runs_fill",
+    "seist_stream_peaks_work_bytes",
     "seist_sizeof_ragged_step", "seist_ragged_window", "seist_ragged_stack", "seist_ragged_emit", "seist_ragged_keep", "seist_ragged_ext",
     "seist_ragged_peaks", "seist_ragged_peaks_fill", "seist_ragged_runs", "seist_ragged_runs_fill",
     "seist_ragged_history", "seist_ragged_event_windows",

@@ -467,22 +467,6 @@ __global__ void __launch_bounds__(ST_NT) stream_keep_kernel(SeistStreamStep p, c
   if (i < keep) tail_out[(size_t)blockIdx.y * p.W + i] = ss_raw(p, tail, chunk, s, c, p.r1 - keep + i);
 }
 
-// ---- raw history of a characterised stream (DESIGN §4.18) ----------------------------------------------------------
-// out (S, C, n_out), row (s, c) = samples [h0_out, h0_out + n_out) of held (S, C, n_held, base h0_held) followed by the
-// chunk (S, C, n); j = h0_out - h0_held + i indexes held ++ chunk.  Every read is range-checked (0.0f outside).
-__global__ void __launch_bounds__(ST_NT) stream_history_kernel(const float* __restrict__ held, long long n_held,
-                                                               const float* __restrict__ chunk, long long n, long long shift,
-                                                               long long n_out, float* __restrict__ out) {
-  const long long i = (long long)blockIdx.x * ST_NT + threadIdx.x;
-  if (i >= n_out) return;
-  const size_t row = blockIdx.y;
-  const long long j = shift + i;
-  float v = 0.f;
-  if (j >= 0 && j < n_held) v = held[row * (size_t)n_held + (size_t)j];
-  else if (j >= n_held && j - n_held < n) v = chunk[row * (size_t)n + (size_t)(j - n_held)];
-  out[row * (size_t)n_out + (size_t)i] = v;
-}
-
 // stack_batch_kernel for the call's windows j0 .. j0 + nb - 1 into acc ([f0, r1)).  A sample that is not new continues
 // from acc when an earlier batch of the call covered it (the station's part of the batch starts after the call's first
 // window: the window before it covers t), else from carry ([f0, r0), earlier calls)
@@ -538,94 +522,10 @@ __global__ void __launch_bounds__(ST_NT) stream_emit_kernel(SeistStreamStep p, c
   }
 }
 
-// pending candidates of the previous call ([nclosed, ncand) of its rows) to the front of this call's rows, rebased
-__global__ void __launch_bounds__(ST_NT) pend_move_kernel(const int* __restrict__ pci, const float* __restrict__ pcv, int pcapc,
-                                                          const int* __restrict__ pnclosed, const int* __restrict__ pncand, long long delta,
-                                                          int* __restrict__ cidx, float* __restrict__ cval, int capc, int* __restrict__ npend) {
-  const int s = blockIdx.y;
-  const int a = pci ? pnclosed[s] : 0, m = pci ? pncand[s] - a : 0;
-  if (blockIdx.x == 0 && threadIdx.x == 0) npend[s] = m;
-  for (int j = blockIdx.x * ST_NT + threadIdx.x; j < m; j += gridDim.x * ST_NT) {
-    cidx[(size_t)s * capc + j] = (int)(pci[(size_t)s * pcapc + a + j] - delta);
-    cval[(size_t)s * capc + j] = pcv[(size_t)s * pcapc + a + j];
-  }
-}
-
-// per row: ncand = pending + new; the closed prefix ends before the last cluster unless its last candidate c has
-// c + mpd <= lim (no later candidate can join it); info = (pending count, global index of the first pending one)
-__global__ void __launch_bounds__(ST_NT) close_scan_kernel(const int* __restrict__ npend, const int* __restrict__ nnew, const int* __restrict__ cidx,
-                                                           int capc, int mpd, long long lim, long long base, int* __restrict__ ncand,
-                                                           int* __restrict__ nclosed, long long* __restrict__ info) {
-  __shared__ int last_s;
-  const int s = blockIdx.x, n = npend[s] + nnew[s];
-  const int* ci = cidx + (size_t)s * capc;
-  if (threadIdx.x == 0) last_s = 0;
-  __syncthreads();
-  for (int top = n - 1; top >= 1; top -= ST_NT) {            // the last cluster start, searched from the end
-    const int j = top - (int)threadIdx.x;
-    const bool f = j >= 1 && ci[j] - ci[j - 1] > mpd;
-    if (f) atomicMax(&last_s, j);
-    if (__syncthreads_or(f)) break;
-  }
-  if (threadIdx.x == 0) {
-    const int nc = n == 0 || (long long)ci[n - 1] + mpd <= lim ? n : last_s;
-    ncand[s] = n;
-    nclosed[s] = nc;
-    info[s] = n - nc;
-    info[gridDim.x + s] = nc < n ? base + ci[nc] : LLONG_MAX;
-  }
-}
-
 // runs of a streamed row: position p closes a run at p - 1 (sr_off) or opens one at p (sr_on); x[lo - 1] is the last
 // sample of the previous stretch
 __device__ __forceinline__ bool sr_off(const float* x, int p, float thr) { return x[p - 1] > thr && !(x[p] > thr); }
 __device__ __forceinline__ bool sr_on(const float* x, int p, float thr) { return x[p] > thr && !(x[p - 1] > thr); }
-
-__global__ void __launch_bounds__(ST_NT) srun_count_kernel(const float* __restrict__ prob, long long n_stride, int lo, int hi, float thr,
-                                                           int* __restrict__ blk, int nblk, const long long* __restrict__ open_in,
-                                                           long long* __restrict__ open_out) {
-  __shared__ int warp_s[ST_NT / 32];
-  const float* x = prob + blockIdx.y * n_stride;
-  const int a = lo + blockIdx.x * ST_CH;
-  int n = 0;
-  for (int i = a + threadIdx.x; i < min(a + ST_CH, hi + 1); i += ST_NT) n += sr_off(x, i, thr);
-  n = st_block_count(n, warp_s);
-  if (threadIdx.x == 0) {
-    blk[(size_t)blockIdx.y * nblk + blockIdx.x] = n;
-    if (blockIdx.x == 0) open_out[blockIdx.y] = x[hi] > thr ? open_in[blockIdx.y] : -1;   // raised by srun_fill on a new start
-  }
-}
-
-// blk: exclusive counts of run ends before each block.  The run ending at the k-th end of the row is pair offsets[s] + k;
-// the carried open run is the first of them.
-__global__ void __launch_bounds__(ST_NT) srun_fill_kernel(const float* __restrict__ prob, long long n_stride, int lo, int hi, float thr,
-                                                          long long g0, const int* __restrict__ blk, int nblk,
-                                                          const long long* __restrict__ offsets, const long long* __restrict__ open_in,
-                                                          long long* __restrict__ open_out, long long* __restrict__ pairs) {
-  __shared__ int warp_s[ST_NT / 32];
-  const float* x = prob + blockIdx.y * n_stride;
-  const int a = lo + blockIdx.x * ST_CH;
-  const long long end = offsets[blockIdx.y + 1];
-  if (blockIdx.x == 0 && threadIdx.x == 0 && open_in[blockIdx.y] >= 0 && end > offsets[blockIdx.y])
-    pairs[offsets[blockIdx.y] * 2] = open_in[blockIdx.y];
-  const bool open_end = x[hi] > thr;
-  long long off_base = offsets[blockIdx.y] + blk[(size_t)blockIdx.y * nblk + blockIdx.x];
-  long long on_base = off_base + (x[a - 1] > thr ? 1 : 0);    // a run open into the block ends before the next starts
-  for (int i0 = a; i0 < min(a + ST_CH, hi + 1); i0 += ST_NT) {
-    const int i = i0 + threadIdx.x;
-    const bool fon = i <= hi && sr_on(x, i, thr), foff = i <= hi && sr_off(x, i, thr);
-    int ton, toff;
-    const int ron = st_block_rank(fon, warp_s, ton);
-    const int roff = st_block_rank(foff, warp_s, toff);
-    if (foff) pairs[(off_base + roff) * 2 + 1] = g0 + i - 1;
-    if (fon) {
-      if (on_base + ron < end) pairs[(on_base + ron) * 2] = g0 + i;
-      else if (open_end) atomicMax(&open_out[blockIdx.y], g0 + i);
-    }
-    on_base += ton;
-    off_base += toff;
-  }
-}
 
 // ---- ragged streams: stations that advance at different rates (DESIGN §4.19) ----------------------------------------
 // One SeistRaggedStep per call; the per-station counts are device arrays, the call's data packed by the prefix arrays.
@@ -854,7 +754,8 @@ __global__ void __launch_bounds__(ST_NT) ragged_ext_kernel(const float* __restri
   if (i == m || i == m + 1) look_out[((size_t)s * C + c) * 2 + (size_t)(i - m)] = v;
 }
 
-// pend_move_kernel with a rebase per row
+// pending candidates of the previous call ([nclosed, ncand) of its rows) to the front of this call's rows, rebased by
+// -delta[s]
 __global__ void __launch_bounds__(ST_NT) rg_pend_move_kernel(const int* __restrict__ pci, const float* __restrict__ pcv, int pcapc,
                                                              const int* __restrict__ pnclosed, const int* __restrict__ pncand,
                                                              const long long* __restrict__ delta, int* __restrict__ cidx,
@@ -919,7 +820,8 @@ __global__ void __launch_bounds__(ST_NT) rg_cand_fill_kernel(const float* __rest
   }
 }
 
-// close_scan_kernel with lim and base per row
+// per row: ncand = pending + new; the closed prefix ends before the last cluster unless its last candidate c has
+// c + mpd <= lim[s] (no later candidate can join it); info = (pending count, global index of the first pending one)
 __global__ void __launch_bounds__(ST_NT) rg_close_scan_kernel(const int* __restrict__ npend, const int* __restrict__ nnew,
                                                               const int* __restrict__ cidx, int capc, int mpd,
                                                               const long long* __restrict__ lim_a, const long long* __restrict__ base_a,
@@ -967,7 +869,7 @@ __global__ void __launch_bounds__(ST_NT) rg_keep_fill_kernel(const int* __restri
   }
 }
 
-// srun_count_kernel over each row's own range [max(lo, 1), min(hi, L - 1)]
+// the run ends in each row's own range [max(lo, 1), min(hi, L - 1)], per block; open_out = the open run carried past it
 __global__ void __launch_bounds__(ST_NT) rg_srun_count_kernel(const float* __restrict__ ext, const long long* __restrict__ ext_off, int C,
                                                               int ch, const long long* __restrict__ lo_a, const long long* __restrict__ hi_a,
                                                               float thr, int* __restrict__ blk, int nblk, const long long* __restrict__ open_in,
@@ -987,7 +889,8 @@ __global__ void __launch_bounds__(ST_NT) rg_srun_count_kernel(const float* __res
   }
 }
 
-// srun_fill_kernel with lo, hi and g0 per row
+// blk: exclusive counts of run ends before each block.  The run ending at the k-th end of row s is pair offsets[s] + k;
+// the carried open run is the first of them.  Pairs are global (g0[s] + position).
 __global__ void __launch_bounds__(ST_NT) rg_srun_fill_kernel(const float* __restrict__ ext, const long long* __restrict__ ext_off, int C,
                                                              int ch, const long long* __restrict__ lo_a, const long long* __restrict__ hi_a,
                                                              float thr, const long long* __restrict__ g0_a, const int* __restrict__ blk,
@@ -1614,105 +1517,9 @@ int seist_stream_keep(const SeistStreamStep* step, const float* tail_raw, const 
   return check_launch("stream_keep");
 }
 
-int seist_stream_history(const float* held, int64_t h0_held, int64_t n_held, const float* chunk, int64_t n, int64_t h0_out,
-                         int32_t S, int32_t C, float* out, int64_t out_capacity, void* stream) {
-  const long long n_out = h0_held + n_held + n - h0_out;
-  if (S <= 0 || C <= 0 || (long long)S * C > 65535 || h0_held < 0 || n_held < 0 || n < 0 || h0_out < h0_held || n_out < 0 ||
-      n_out > INT32_MAX || (n_held > 0 && !held) || (n > 0 && !chunk) || out_capacity < (long long)S * C * n_out ||
-      (n_out > 0 && (!out || out == held || out == chunk))) {
-    set_error("stream_history: bad arguments (0 <= h0_held <= h0_out <= h0_held + n_held + n, output length < 2^31, "
-              "S * C <= 65535, out_capacity >= S * C * output length, out distinct from held and chunk)");
-    return -1;
-  }
-  if (n_out == 0) return 0;
-  stream_history_kernel<<<dim3((unsigned)((n_out + ST_NT - 1) / ST_NT), (unsigned)(S * C)), ST_NT, 0, (cudaStream_t)stream>>>(
-      held, n_held, chunk, n, h0_out - h0_held, n_out, out);
-  note_launch();
-  return check_launch("stream_history");
-}
-
 int64_t seist_stream_peaks_work_bytes(int32_t S, int32_t capc, int64_t L) {
   if (S <= 0 || capc < 1 || L < 2 || L > INT32_MAX) return -1;
   return (int64_t)StreamPeakWork(nullptr, S, capc, L).bytes;
-}
-
-int seist_stream_peaks(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float mph,
-                       int32_t min_peak_dist, int64_t lim, int64_t base, int32_t ishift, void* work, int32_t capc,
-                       const void* prev, int32_t prev_capc, int64_t prev_L, int64_t delta, int32_t max_pend, int64_t* counts,
-                       int64_t* info, void* stream) {
-  if (!ext || !work || !counts || !info || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || channel < 0 || channel >= C ||
-      lo < 1 || hi > L - 2 || min_peak_dist <= 1 || ishift < 0 || max_pend < 0 || capc < max_pend + (int)(L / 2) + 1 ||
-      (prev && (prev_capc < 1 || prev_L < 2 || prev_L > INT32_MAX))) {
-    set_error("stream_peaks: bad arguments (1 <= lo, hi <= L - 2, S <= 65535, min_peak_dist > 1, capc >= max_pend + L / 2 + 1)");
-    return -1;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  const StreamPeakWork w(work, S, capc, L);
-  const float* x = ext + (size_t)channel * L;
-  const long long ns = (long long)C * L;
-  const int nb = std::max(1, st_nblk(hi - lo + 1)), nbc = st_nblk(capc);
-  const StreamPeakWork pw(prev, S, prev ? prev_capc : 1, prev ? prev_L : 2);
-  pend_move_kernel<<<dim3(std::max(1, (max_pend + ST_NT - 1) / ST_NT), S), ST_NT, 0, st>>>(
-      prev ? pw.cidx : nullptr, pw.cval, prev_capc, pw.nclosed, pw.ncand, delta, w.cidx, w.cval, capc, w.npend);
-  cand_count_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(x, ns, lo, hi, mph, w.blk, nb);
-  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nb, w.nnew, nullptr);
-  cand_fill_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(x, ns, lo, hi, mph, w.blk, nb, w.npend, ishift, capc, w.cidx, w.cval);
-  close_scan_kernel<<<S, ST_NT, 0, st>>>(w.npend, w.nnew, w.cidx, capc, min_peak_dist, lim, base, w.ncand, w.nclosed, (long long*)info);
-  cluster_kernel<<<dim3((capc + CL_SEG - 1) / CL_SEG, S), ST_NT, 0, st>>>(w.nclosed, capc, w.cidx, w.cval, w.state, min_peak_dist);
-  keep_count_kernel<<<dim3(nbc, S), ST_NT, 0, st>>>(w.nclosed, capc, w.state, w.blk, nbc);
-  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(w.blk, nbc, w.nkeep, (long long*)counts);
-  for (int i = 0; i < 8; ++i) note_launch();
-  return check_launch("stream_peaks");
-}
-
-int seist_stream_peaks_fill(int32_t S, int64_t L, const void* work, int32_t capc, int64_t base, const int64_t* offsets,
-                            int64_t* index, float* value, void* stream) {
-  if (!work || !offsets || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || capc < 1) {
-    set_error("stream_peaks_fill: bad arguments (the work buffer of the seist_stream_peaks call)");
-    return -1;
-  }
-  const StreamPeakWork w(work, S, capc, L);
-  const int nbc = st_nblk(capc);
-  keep_fill_kernel<<<dim3(nbc, S), ST_NT, 0, (cudaStream_t)stream>>>(w.nclosed, capc, w.cidx, w.cval, w.state, w.blk, nbc,
-                                                                     (const long long*)offsets, base, (long long*)index, value);
-  note_launch();
-  return check_launch("stream_peaks_fill");
-}
-
-int seist_stream_runs(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi, float threshold,
-                      const int64_t* open_in, int64_t* open_out, void* work, int64_t work_bytes, int64_t* counts, void* stream) {
-  if (!ext || !work || !counts || !open_in || !open_out || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || channel < 0 ||
-      channel >= C || lo < 1 || hi > L - 1 || hi < lo - 1 || work_bytes < seist_runs_work_bytes(S, L)) {
-    set_error("stream_runs: bad arguments (1 <= lo, lo - 1 <= hi <= L - 1, S <= 65535, work >= seist_runs_work_bytes)");
-    return -1;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  int* total = (int*)work;
-  int* blk = (int*)((char*)work + st_align(sizeof(int) * S));
-  const int nb = std::max(1, st_nblk(hi - lo + 1));
-  srun_count_kernel<<<dim3(nb, S), ST_NT, 0, st>>>(ext + (size_t)channel * L, (long long)C * L, lo, hi, threshold, blk, nb,
-                                                  (const long long*)open_in, (long long*)open_out);
-  scan_rows_kernel<<<S, ST_SCAN_NT, 0, st>>>(blk, nb, total, (long long*)counts);
-  note_launch();
-  note_launch();
-  return check_launch("stream_runs");
-}
-
-int seist_stream_runs_fill(const float* ext, int32_t S, int32_t C, int32_t channel, int64_t L, int32_t lo, int32_t hi,
-                           float threshold, int64_t g0, const int64_t* open_in, int64_t* open_out, const void* work,
-                           int64_t work_bytes, const int64_t* offsets, int64_t* pairs, void* stream) {
-  if (!ext || !work || !offsets || !open_in || !open_out || S <= 0 || S > 65535 || L < 2 || L > INT32_MAX || channel < 0 ||
-      channel >= C || lo < 1 || hi > L - 1 || hi < lo - 1 || work_bytes < seist_runs_work_bytes(S, L)) {
-    set_error("stream_runs_fill: bad arguments (the work buffer of the seist_stream_runs call)");
-    return -1;
-  }
-  const int* blk = (const int*)((const char*)work + st_align(sizeof(int) * S));
-  const int nb = std::max(1, st_nblk(hi - lo + 1));
-  srun_fill_kernel<<<dim3(nb, S), ST_NT, 0, (cudaStream_t)stream>>>(ext + (size_t)channel * L, (long long)C * L, lo, hi, threshold, g0,
-                                                                    blk, nb, (const long long*)offsets, (const long long*)open_in,
-                                                                    (long long*)open_out, (long long*)pairs);
-  note_launch();
-  return check_launch("stream_runs_fill");
 }
 
 uint64_t seist_sizeof_ragged_step(void) { return sizeof(SeistRaggedStep); }

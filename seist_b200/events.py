@@ -201,24 +201,6 @@ class EventCharacterizer:
         return GapCharacterizedStream(self, annotator, n_stations)
 
 
-def stream_history_(out: torch.Tensor, held: torch.Tensor, h0_held: int, chunk: torch.Tensor | None, h0_out: int) -> torch.Tensor:
-    """The raw samples [h0_out, h0_held + held.shape[2] + n) of every row, from held (S, C, n_held: samples h0_held ..)
-    followed by chunk (S, C, n), written packed into the flat float32 buffer out -> the (S, C, n_out) view of it."""
-    _dense(held, (None, None, None), "held samples")
-    S, C, n_held = held.shape
-    n = 0 if chunk is None else chunk.shape[2]
-    if chunk is not None:
-        _dense(chunk, (S, C, None), "chunk", held.device)
-    _dense(out, (None,), "history buffer", held.device)
-    n_out = h0_held + n_held + n - h0_out
-    if not (0 <= h0_held <= h0_out and 0 <= n_out <= _I32_MAX and S * C * n_out <= out.numel()):
-        raise ValueError(f"need 0 <= h0_held <= h0_out, an output of 0 .. 2^31 - 1 samples and a buffer of S * C * n_out floats, "
-                         f"got h0_held {h0_held}, h0_out {h0_out}, n_out {n_out}, buffer {out.numel()}")
-    _lib.check(_lib.lib().seist_stream_history(held.data_ptr() if n_held else None, h0_held, n_held, chunk.data_ptr() if n else None, n,
-                                               h0_out, S, C, out.data_ptr(), out.numel(), _s()), "seist_stream_history")
-    return out[:S * C * n_out].view(S, C, n_out)
-
-
 def _check_pair(ch: EventCharacterizer, ann: ContinuousAnnotator):
     """A characteriser and an annotator that can stream together (raises ValueError otherwise)."""
     dev = next(ann.model.parameters()).device
@@ -251,8 +233,9 @@ class CharacterizedStream:
         self.ch = ch
         self.stream = ann.open_stream(n_stations)
         self.S, self.C, self.device = self.stream.S, self.stream.C, self.stream.device
-        self.buf = [torch.empty(0, device=self.device), torch.empty(0, device=self.device)]
-        self.history = self.buf[0].view(self.S, self.C, 0)
+        self.buf = [torch.zeros(1, device=self.device), torch.zeros(1, device=self.device)]
+        self.desc = torch.zeros(2 * self.S + 1, dtype=torch.int64, device=self.device)   # h0 (S,), off (S + 1,) of buf[0]
+        self.history = self.buf[0][:0].view(self.S, self.C, 0)
         self.h0 = self.R = 0
         self.keep = 0            # the retention bound after the last call
 
@@ -273,14 +256,13 @@ class CharacterizedStream:
         n = chunk.shape[2] if isinstance(chunk, torch.Tensor) and chunk.dim() == 3 else 0
         if not self.closed and self.R + n - self.keep > _I32_MAX:
             raise ValueError(f"the history would hold {self.R + n - self.keep} samples per row, more than 2^31 - 1")
+        S, C = self.S, self.C
+        hp = ragged_history_plan(np.full(S, self.h0), np.full(S, self.R), np.full(S, n), np.full(S, self.keep)) if n else None
         out = self.stream.push(chunk)              # validates the chunk before any launch
         if n:
-            need = self.S * self.C * (self.R + n - self.keep)
-            if self.buf[1].numel() < need:
-                self.buf[1] = torch.empty(max(need, 2 * self.buf[1].numel()), device=self.device)
-            self.history = stream_history_(self.buf[1], self.history, self.h0, chunk, self.keep)
-            self.buf.reverse()
+            self.desc = push_history_(self.buf, self.desc, hp, chunk, n * np.arange(S + 1), C)   # the (S, C, n) chunk is packed
             self.h0, self.R = self.keep, self.R + n
+            self.history = self.buf[0][:S * C * (self.R - self.h0)].view(S, C, self.R - self.h0)
         return self._finish(out)
 
     @torch.no_grad()
@@ -289,7 +271,7 @@ class CharacterizedStream:
 
     def _finish(self, out: StreamOutput) -> CharacterizedOutput:
         pk = self.stream.picker
-        self.keep = max(self.keep, min(pk.first_pend[1], pk.F - 1) - self.ch.anchor)
+        self.keep = max(self.keep, int(min(pk.first_pend[1].min(), pk.F.min() - 1)) - self.ch.anchor)
         index, _, offsets = out.ppk
         rel = index - self.h0 if index.numel() else index
         return CharacterizedOutput(out, self.ch._run(self.history, rel, offsets))
@@ -339,6 +321,21 @@ def ragged_history_(out: torch.Tensor, held: torch.Tensor, held_h0: torch.Tensor
                                                chunk_off.data_ptr(), chunk.numel(), h0_out.data_ptr(), out_off.data_ptr(), S, int(C),
                                                int(max_len), out.data_ptr(), out.numel(), _s()), "seist_ragged_history")
     return out
+
+
+def push_history_(buf: list, desc: torch.Tensor, hp: dict, chunk: torch.Tensor, chunk_off, C: int) -> torch.Tensor:
+    """One history step of a characterised stream: the histories planned by `ragged_history_plan` (hp) written into
+    buf[1], grown when too small, from the held histories in buf[0] (device h0 (S,) and offsets (S + 1,) in desc) followed
+    by each station's block of the packed chunk (C * chunk_off[s], host int64 (S + 1,)); then the two buffers swap.
+    Returns the device h0 and offsets (2S + 1,) of the histories now in buf[0]."""
+    S, dev = hp["h0"].size, desc.device
+    need = C * int(hp["off"][-1])
+    if buf[1].numel() < need:
+        buf[1] = torch.empty(max(need, 2 * buf[1].numel()), device=dev)
+    d = _upload(np.concatenate([hp["h0"], hp["off"], chunk_off]), dev)   # the history descriptors
+    ragged_history_(buf[1], buf[0], desc[:S], desc[S:], chunk, d[2 * S + 1:], d[:S], d[S:2 * S + 1], C, int(hp["len"].max()))
+    buf.reverse()
+    return d[:2 * S + 1]
 
 
 def ragged_event_windows_(xs, hist: torch.Tensor, hist_h0: torch.Tensor, hist_off: torch.Tensor, index: torch.Tensor,
@@ -416,15 +413,7 @@ class RaggedCharacterizedStream:
             raise ValueError(f"the histories of stations {s} would hold {hp['len'][s].tolist()} samples, more than 2^31 - 1")
         out = self.stream._call(plan, chunk, False)
         if n.any():
-            S = self.S
-            need = self.C * int(hp["off"][-1])
-            if self.buf[1].numel() < need:
-                self.buf[1] = torch.empty(max(need, 2 * self.buf[1].numel()), device=self.device)
-            dev = _upload(np.concatenate([hp["h0"], hp["off"], plan["chunk_off"]]), self.device)   # the history descriptors
-            ragged_history_(self.buf[1], self.buf[0], self.desc[:S], self.desc[S:], chunk, dev[2 * S + 1:], dev[:S], dev[S:2 * S + 1],
-                            self.C, int(hp["len"].max()))
-            self.buf.reverse()
-            self.desc = dev[:2 * S + 1]
+            self.desc = push_history_(self.buf, self.desc, hp, chunk, plan["chunk_off"], self.C)
             self.h0 = hp["h0"]
         self.R = hp["R"]
         return self._finish(out)

@@ -226,108 +226,6 @@ class StreamOutput(NamedTuple):
     det: tuple
 
 
-class PickStream:
-    """The probability side of a stream: takes the final (S, 3, m) probabilities of a record in order, stretch after
-    stretch, and returns the picks and detection runs that closed (DESIGN §4.16).  A candidate is decided once the
-    sample after it is final; a cluster of candidates (consecutive gaps <= min_peak_dist) is resolved once its last
-    candidate c has c + min_peak_dist <= F - 2 (F: the final samples so far), so a pick waits for its cluster to close.
-    A run closes once the sample after its end is final.  `t0` is the global index of the first sample."""
-
-    def __init__(self, n_stations: int, device, min_peak_dist: int, ppk_threshold: float = 0.3, spk_threshold: float = 0.3,
-                 det_threshold: float = 0.5, t0: int = 0):
-        if min_peak_dist is None or int(min_peak_dist) <= 1:
-            raise ValueError(f"min_peak_dist must be > 1 samples, got {min_peak_dist}")
-        if int(n_stations) < 1:
-            raise ValueError(f"need at least one station, got {n_stations}")
-        self.S, self.device, self.mpd = int(n_stations), torch.device(device), int(min_peak_dist)
-        if self.device.type == "cuda" and self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
-        self.thr = (float(det_threshold), float(ppk_threshold), float(spk_threshold))
-        self.t0 = self.F = int(t0)
-        self.closed = False
-        self.look = torch.full((self.S, 3, 2), float("-inf"), device=self.device)      # the last two final samples
-        self.open = torch.full((self.S,), -1, dtype=torch.int64, device=self.device)   # start of each open run
-        self.pend = {1: None, 2: None}        # per pick channel: (work, capc, L, base) of the previous call
-        self.max_pend = {1: 0, 2: 0}
-        self.first_pend = {1: _I64_MAX, 2: _I64_MAX}
-
-    def push(self, probs: torch.Tensor):
-        """The next final stretch (S, 3, m), m >= 0 -> (ppk, spk, det) that closed."""
-        return self._step(probs, False)
-
-    def close(self, probs: torch.Tensor | None = None):
-        """The last stretch: every pending cluster and open run closes; sample F - 1 ends the record."""
-        if probs is None:
-            probs = torch.empty(self.S, 3, 0, device=self.device)
-        return self._step(probs, True)
-
-    def _step(self, probs: torch.Tensor, last: bool):
-        if self.closed:
-            raise RuntimeError("the stream is closed")
-        if not probs.is_cuda:
-            raise RuntimeError("PickStream has no CPU path: the probabilities must live on a CUDA device")
-        _dense(probs, (self.S, 3, None), "probabilities", self.device)
-        S, m = self.S, probs.shape[2]
-        f0, f1 = self.F, self.F + m
-        if last and f1 - self.t0 < 3:
-            raise ValueError(f"a record of {f1 - self.t0} samples is too short to pick")
-        lib, dev = _lib.lib(), self.device
-        parts = [self.look, probs] + ([torch.full((S, 3, 1), float("-inf"), device=dev)] if last else [])
-        ext = torch.cat(parts, 2)
-        L, g0 = ext.shape[2], f0 - 2
-        if L > _I32_MAX:
-            raise ValueError(f"a stretch of {m} samples is too long for one call")
-        staged = []
-        for ch in (1, 2):
-            prev = self.pend[ch]
-            base = min(g0, self.first_pend[ch])
-            if f1 - base >= _I32_MAX - 2:
-                raise RuntimeError(f"a cluster of candidates spans more than 2^31 samples (channel {ch})")
-            capc = self.max_pend[ch] + L // 2 + 1
-            nbytes = lib.seist_stream_peaks_work_bytes(S, capc, L)
-            work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            counts = torch.empty(S, dtype=torch.int64, device=dev)
-            info = torch.empty(2 * S, dtype=torch.int64, device=dev)
-            lim = _I64_MAX >> 1 if last else f1 - 2 - base
-            _lib.check(lib.seist_stream_peaks(ext.data_ptr(), S, 3, ch, L, max(1, 3 - (f0 - self.t0)), m, self.thr[ch], self.mpd, lim,
-                                              base, g0 - base, work.data_ptr(), capc,
-                                              prev[0].data_ptr() if prev else None, prev[1] if prev else 0, prev[2] if prev else 0,
-                                              base - prev[3] if prev else 0, self.max_pend[ch], counts.data_ptr(), info.data_ptr(),
-                                              _s()), "seist_stream_peaks")
-            staged.append((work, capc, base, _offsets(counts), info))
-        hi = m + 2 if last else m + 1
-        rbytes = lib.seist_runs_work_bytes(S, L)
-        rwork = torch.empty(rbytes, dtype=torch.uint8, device=dev)
-        rcounts = torch.empty(S, dtype=torch.int64, device=dev)
-        open_out = torch.empty(S, dtype=torch.int64, device=dev)
-        _lib.check(lib.seist_stream_runs(ext.data_ptr(), S, 3, 0, L, 2, hi, self.thr[0], self.open.data_ptr(), open_out.data_ptr(),
-                                         rwork.data_ptr(), rbytes, rcounts.data_ptr(), _s()), "seist_stream_runs")
-        roff = _offsets(rcounts)
-        tot = torch.cat([staged[0][3][-1:], staged[1][3][-1:], roff[-1:], staged[0][4], staged[1][4]]).tolist()   # the one host sync
-        out = []
-        for i, (ch, (work, capc, base, off, info)) in enumerate(zip((1, 2), staged)):
-            n = tot[i]
-            index = torch.empty(n, dtype=torch.int64, device=dev)
-            value = torch.empty(n, dtype=torch.float32, device=dev)
-            if n:
-                _lib.check(lib.seist_stream_peaks_fill(S, L, work.data_ptr(), capc, base, off.data_ptr(), index.data_ptr(),
-                                                       value.data_ptr(), _s()), "seist_stream_peaks_fill")
-            out.append((index, value, off))
-            o = 3 + 2 * S * i
-            self.max_pend[ch] = max(tot[o:o + S])
-            self.first_pend[ch] = min(tot[o + S:o + 2 * S])
-            self.pend[ch] = (work, capc, L, base)
-        pairs = torch.empty(tot[2], 2, dtype=torch.int64, device=dev)
-        _lib.check(lib.seist_stream_runs_fill(ext.data_ptr(), S, 3, 0, L, 2, hi, self.thr[0], g0, self.open.data_ptr(),
-                                              open_out.data_ptr(), rwork.data_ptr(), rbytes, roff.data_ptr(),
-                                              pairs.data_ptr() if pairs.numel() else None, _s()), "seist_stream_runs_fill")
-        self.open = open_out
-        self.look = ext[:, :, m:m + 2].clone()
-        self.F = f1
-        self.closed = last
-        return out[0], out[1], (pairs, roff)
-
-
 class ContinuousStream:
     """A record annotated chunk by chunk (`ContinuousAnnotator.open_stream`).  `push(chunk)` takes (S, C, n) float32 on the
     model's device, any n >= 0; `close()` ends the record.  Each returns a StreamOutput; concatenated, their probs equal
@@ -343,8 +241,8 @@ class ContinuousStream:
         self.carry = [torch.zeros(self.S, 3, W, device=self.device) for _ in range(2)]
         self.R = self.F = self.k = 0
         self.forwards = 0
-        self.picker = PickStream(self.S, self.device, ann.min_peak_dist, ann.thresholds["ppk"], ann.thresholds["spk"],
-                                 ann.thresholds["det"])
+        self.picker = RaggedPickStream(self.S, self.device, ann.min_peak_dist, ann.thresholds["ppk"], ann.thresholds["spk"],
+                                       ann.thresholds["det"])
 
     @property
     def closed(self) -> bool:
@@ -564,9 +462,13 @@ class RaggedStreamOutput(NamedTuple):
 
 
 class RaggedPickStream:
-    """PickStream whose rows take stretches of different lengths: `push(stretches)` takes S (3, m_s) float32 tensors, any
-    m_s >= 0; each row keeps its own final count F_s and is decided by the §4.16 rules on its own.  `t0` (an int or one
-    per row) is the global index of each row's first sample."""
+    """The probability side of a stream: takes the final probabilities of S rows in order, stretch after stretch, and
+    returns the picks and detection runs that closed (DESIGN §4.16, §4.19).  `push(probs)` takes one (S, 3, m) float32
+    tensor (every row a stretch of m samples) or S (3, m_s) float32 tensors, any m, m_s >= 0; each row keeps its own final
+    count F_s.  A candidate is decided once the sample after it is final; a cluster of candidates (consecutive gaps <=
+    min_peak_dist) is resolved once its last candidate c has c + min_peak_dist <= F_s - 2, so a pick waits for its cluster
+    to close.  A run closes once the sample after its end is final.  `t0` (an int or one per row) is the global index of
+    each row's first sample."""
 
     def __init__(self, n_stations: int, device, min_peak_dist: int, ppk_threshold: float = 0.3, spk_threshold: float = 0.3,
                  det_threshold: float = 0.5, t0=0):
@@ -589,7 +491,8 @@ class RaggedPickStream:
         self._none = torch.zeros(1, device=self.device)
 
     def push(self, probs):
-        """The next final stretch of every row (a sequence of S (3, m_s) tensors) -> (ppk, spk, det) that closed."""
+        """The next final stretch of every row (one (S, 3, m) tensor or a sequence of S (3, m_s) tensors) -> (ppk, spk, det)
+        that closed."""
         return self._stretches(probs, False)
 
     def close(self, probs=None):
@@ -601,15 +504,23 @@ class RaggedPickStream:
     def _stretches(self, probs, last: bool):
         if self.closed:
             raise RuntimeError("the stream is closed")
-        if len(probs) != self.S:
-            raise ValueError(f"expected {self.S} stretches, got {len(probs)}")
-        for p in probs:
-            if not p.is_cuda:
-                raise RuntimeError("RaggedPickStream has no CPU path: the probabilities must live on a CUDA device")
-            _dense(p, (3, None), "probabilities", self.device)
-        m = np.array([p.shape[1] for p in probs], dtype=np.int64)
+        dense = torch.is_tensor(probs)             # one stretch of m samples per row, already packed
+        if dense:
+            _dense(probs, (self.S, 3, None), "probabilities", self.device)
+            m = np.full(self.S, probs.shape[2], np.int64)
+        else:
+            if len(probs) != self.S:
+                raise ValueError(f"expected {self.S} stretches, got {len(probs)}")
+            for p in probs:
+                if not p.is_cuda:
+                    raise RuntimeError("RaggedPickStream has no CPU path: the probabilities must live on a CUDA device")
+                _dense(p, (3, None), "probabilities", self.device)
+            m = np.array([p.shape[1] for p in probs], dtype=np.int64)
         host, meta = self._plan(m, last)
-        flat = torch.cat([p.reshape(-1) for p in probs]) if m.sum() else self._none
+        if not m.any():
+            flat = self._none
+        else:
+            flat = probs.view(-1) if dense else torch.cat([p.reshape(-1) for p in probs])
         return self._run(flat, m, last, host, _upload(host, self.device), meta)
 
     def _plan(self, m: np.ndarray, last: bool):

@@ -1,4 +1,4 @@
-"""-m gpu: continuous records streamed chunk by chunk (seist_b200/stream.py ContinuousStream / PickStream, csrc/stream.cu)
+"""-m gpu: continuous records streamed chunk by chunk (seist_b200/stream.py ContinuousStream / RaggedPickStream, csrc/stream.cu)
 against the streaming oracle (tests/stream_chunks_ref.py) call by call, and end to end against `annotate` + whole-record
 picking on the same record."""
 import numpy as np
@@ -25,7 +25,7 @@ def model():
 
 
 def _np(out):
-    """A StreamOutput (or a PickStream result) as numpy."""
+    """A StreamOutput (or a RaggedPickStream result) as numpy."""
     return tuple(tuple(t.cpu().numpy() for t in part) if isinstance(part, tuple) else part.cpu().numpy() if torch.is_tensor(part)
                  else part for part in out)
 
@@ -57,7 +57,7 @@ def _drive_helpers(rec, split, W, P, B, mode, fn, mpd, thr):
     dev = "cuda"
     tail = [torch.zeros(S, C, W, device=dev) for _ in range(2)]
     carry = [torch.zeros(S, 3, W, device=dev) for _ in range(2)]
-    picker = ST.PickStream(S, dev, mpd, thr[1], thr[2], thr[0])
+    picker = ST.RaggedPickStream(S, dev, mpd, thr[1], thr[2], thr[0])
     R = F = k = 0
     pos = 0
     for n in list(split) + [None]:
@@ -99,7 +99,7 @@ def _drive_helpers(rec, split, W, P, B, mode, fn, mpd, thr):
 
 @pytest.mark.parametrize("mode", ["mean", "max"])
 @pytest.mark.parametrize("W,P,B", [(512, 256, 3), (600, 250, 5)])
-def test_helpers_equal_stream_ref_call_by_call(mode, W, P, B):
+def test_helpers_and_ragged_picker_equal_stream_ref_call_by_call(mode, W, P, B):
     S, C, T = 3, 3, 4 * 600 + 77
     rng = np.random.default_rng(W + P)
     rec = (rng.standard_normal((S, C, T)) * 3 + 1).astype(np.float32)
@@ -122,7 +122,7 @@ def test_helpers_equal_stream_ref_call_by_call(mode, W, P, B):
 def _feed(probs, split, mpd, thr, t0=0):
     S = probs.shape[0]
     ref = PickStreamRef(S, mpd, thr, t0)
-    dev = ST.PickStream(S, "cuda", mpd, thr[1], thr[2], thr[0], t0=t0)
+    dev = ST.RaggedPickStream(S, "cuda", mpd, thr[1], thr[2], thr[0], t0=t0)
     pc = torch.from_numpy(probs).cuda()
     outs, pos = [], 0
     for n in list(split) + [None]:
@@ -136,7 +136,7 @@ def _feed(probs, split, mpd, thr, t0=0):
     return outs
 
 
-def test_probability_stage_long_rows_match_oracle():
+def test_dense_probability_pushes_long_rows_match_oracle():
     probs = _long_probs()
     T = probs.shape[2]
     rng = np.random.default_rng(5)
@@ -150,7 +150,7 @@ def test_probability_stage_long_rows_match_oracle():
         assert np.array_equal(got[3][0], pairs) and np.array_equal(got[3][1], off)
 
 
-def test_probability_stage_crosses_2_31():
+def test_dense_probability_pushes_cross_2_31():
     t0 = (1 << 31) - 40_000
     probs = _long_probs()[:, :, :100_000].copy()
     got = concat(_feed(probs, [30_000, 1, 9_999, 25_000, 7], 50, (0.3, 0.3, 0.1), t0), 4)
@@ -198,7 +198,7 @@ def test_stream_equals_annotate_end_to_end(model, stride, batch):
         assert np.array_equal(got[3][0], SR.detect_all(got[0], 0, 0.3)[0])
 
 
-def test_stream_argument_errors_raise_before_launch(model):
+def test_stream_and_picker_argument_errors_raise_before_launch(model):
     ann = ST.ContinuousAnnotator(model, window=8192, stride=4096, batch=2)
     lib = _lib.lib()
     torch.cuda.synchronize()
@@ -228,8 +228,8 @@ def test_stream_argument_errors_raise_before_launch(model):
     with pytest.raises(ValueError):
         st.close()                                                  # fewer than `window` samples
     with pytest.raises(ValueError):
-        ST.PickStream(2, "cuda", 1)
-    pk = ST.PickStream(2, "cuda", 10)
+        ST.RaggedPickStream(2, "cuda", 1)
+    pk = ST.RaggedPickStream(2, "cuda", 10)
     with pytest.raises(ValueError):
         pk.push(torch.zeros(3, 3, 10, device="cuda"))
     step = ST.stream_step(2, 3, 8192, 4096, 0, 0, 0, 100, 0, 0)

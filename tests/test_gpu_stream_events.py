@@ -1,5 +1,5 @@
-"""-m gpu: the P picks of a streamed record characterised as they close (seist_b200/events.py CharacterizedStream,
-`seist_stream_history` in csrc/stream.cu).  The history kernel against slices of the whole record and the rebased cut
+"""-m gpu: the P picks of a streamed record characterised as they close (seist_b200/events.py CharacterizedStream and
+push_history_, `seist_ragged_history` in csrc/stream.cu).  The history kernel against slices of the whole record and the rebased cut
 bit for bit against the cut of the whole record (bases near 2^40 included); seist_s_dpk streamed with
 seist_s_{pmp,emg,baz,dis} bit-identical per station to `ch(record, pick_phases(annotate(record))["ppk"])`; the launches of
 a call over a plain ContinuousStream; bounded state; argument errors before any launch."""
@@ -28,23 +28,25 @@ def _record(S, C, T, seed):
 
 
 def _history_steps(rec, split, keeps, base):
-    """Drive stream_history_ over rec pushed in `split`, keeping [keep, R) at each step (global indices from `base`)."""
+    """Drive push_history_ as CharacterizedStream does over rec pushed in `split` (one dense (S, C, n) chunk per step),
+    a non-empty push keeping [keep, R) (global indices from `base`) -> per step the (S, C, R - h0) history, h0 and R.
+    The buffers start NaN and large enough for the whole record, so every sample the history shows was written."""
     S, C, T = rec.shape
-    bufs = [torch.empty(0, device="cuda"), torch.empty(0, device="cuda")]
-    hist, h0, R = bufs[0].view(S, C, 0), base, base
+    bufs = [torch.full((S * C * T,), float("nan"), device="cuda") for _ in range(2)]
+    desc = torch.zeros(2 * S + 1, dtype=torch.int64, device="cuda")
+    h0, R = base, base
     for n, keep in zip(split, keeps):
-        need = S * C * (R + n - keep)
-        if bufs[1].numel() < need:
-            bufs[1] = torch.full((max(need, 2 * bufs[1].numel()),), float("nan"), device="cuda")
-        chunk = rec[:, :, R - base:R - base + n].contiguous() if n else None
-        hist = EV.stream_history_(bufs[1], hist, h0, chunk, keep)
-        bufs.reverse()
-        h0, R = keep, R + n
-        yield hist, h0, R
+        if n:
+            hp = EV.ragged_history_plan(np.full(S, h0), np.full(S, R), np.full(S, n), np.full(S, keep))
+            chunk = rec[:, :, R - base:R - base + n].contiguous()
+            desc = EV.push_history_(bufs, desc, hp, chunk, n * np.arange(S + 1), C)
+            h0 = keep
+        R += n
+        yield bufs[0][:S * C * (R - h0)].view(S, C, R - h0), h0, R
 
 
 @pytest.mark.parametrize("base", [0, (1 << 40) - 7000])
-def test_history_and_rebased_cut_equal_the_whole_record(base):
+def test_shared_history_and_rebased_cut_equal_the_whole_record(base):
     S, C, T, W = 5, 3, 30_000, 2048
     rec = _record(S, C, T, 31)
     rec[2, 1, :] = 3.0                                                     # a constant channel
@@ -211,7 +213,7 @@ def test_state_is_bounded(models):
     assert max(mem[25:]) <= max(mem[5:25]), mem
 
 
-def test_argument_errors_raise_before_launch(models):
+def test_stream_and_history_argument_errors_raise_before_launch(models):
     ann = _annotator(models, 4096, batch=2)
     ch = EV.EventCharacterizer({"pmp": models["pmp"]}, window=8192, p_position_ratio=0.3, batch=2)
     lib = _lib.lib()
@@ -251,10 +253,12 @@ def test_argument_errors_raise_before_launch(models):
     before = lib.seist_launch_count()
     with pytest.raises(ValueError):
         cs.close()                                                         # fewer than `window` samples
+    idx = torch.zeros(3, dtype=torch.int64, device="cuda")
     with pytest.raises(ValueError):
-        EV.stream_history_(torch.zeros(10, device="cuda"), torch.zeros(2, 3, 5, device="cuda"), 0, None, 1)   # buffer too small
+        EV.ragged_history_(torch.zeros(0, device="cuda"), torch.zeros(30, device="cuda"), idx[:2], idx, torch.zeros(30, device="cuda"),
+                           idx, idx[:2], idx, 3, 5)                                            # an empty history buffer
     with pytest.raises(ValueError):
-        EV.stream_history_(torch.zeros(100, device="cuda"), torch.zeros(2, 3, 5, device="cuda"), 10, None, 9)  # h0_out < h0_held
+        EV.ragged_history_plan([10, 10], [15, 15], [5, 5], [9, 9])                          # h0_out < h0_held
     assert lib.seist_launch_count() == before
     cs.push(torch.zeros(2, 3, 8192, device="cuda"))
     cs.close()

@@ -130,7 +130,7 @@ def main():
 
     # instrumented pass: CUDA events around every history launch and every cut
     spans = {"history": [], "cut": []}
-    orig = {"history": EV.stream_history_, "cut": EV.event_windows_}
+    orig = {"history": EV.ragged_history_, "cut": EV.event_windows_}
 
     def timed(kind):
         def f(*args, **kw):
@@ -142,11 +142,11 @@ def main():
             return r
         return f
 
-    EV.stream_history_, EV.event_windows_ = timed("history"), timed("cut")
+    EV.ragged_history_, EV.event_windows_ = timed("history"), timed("cut")
     try:
         events()
     finally:
-        EV.stream_history_, EV.event_windows_ = orig["history"], orig["cut"]
+        EV.ragged_history_, EV.event_windows_ = orig["history"], orig["cut"]
     ms = {k: sum(e0.elapsed_time(e1) for e0, e1 in v) for k, v in spans.items()}
 
     name = card()
