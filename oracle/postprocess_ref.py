@@ -11,9 +11,13 @@ Restates, in numpy, for the reference's default configuration (mpd > 1, rising e
   * `Metrics.compute` counters for the tasks ppk / spk / det — utils/metrics.py:141-247.
 `pick_phase` IS pinned: tests/test_cpu_postprocess.py executes the reference's own `_detect_peaks` source (extracted from
 the file with `ast`, nothing else of that module imports here) on random and crafted traces and compares index for index.
-Tie rule: for EQUAL peak heights the reference's order is unspecified (`np.argsort` defaults to an unstable, on x86 SIMD,
-sort; observed here: either index can win).  This restatement and the GPU kernel define it: the larger index first.
-Probability traces of the network have no exact ties on the P/S channels (SURVEY section 0.7).
+Tie rule: the reference ranks candidates with `np.argsort(x[ind])[::-1]`, whose default sort is unstable (on x86 SIMD
+either of two equal heights can win).  This restatement and the GPU kernels are the reference with a STABLE sort: equal
+heights, the larger index first.  tests/test_cpu_peak_ties.py pins that against the reference's own `_detect_peaks` run
+with `np.argsort(kind="stable")` on tie-rich traces (tests/golden/reference_peak_ties.pt).  Ties do occur: quantised
+inputs, sigmoid outputs saturated at 1.0f, plateaus on the detection channel (SURVEY section 0.7).
+NaN rule, pinned by the same fixture: NaN and its two neighbours are never peaks (the reference maps NaN to inf and
+removes them; here every comparison with NaN is false, which gives the same candidates), and a NaN sample is in no run.
 """
 import numpy as np
 
@@ -21,7 +25,7 @@ PAD_PHASE = int(-1e7)
 
 
 def detect_peaks_topk(x: np.ndarray, mph: float, mpd: int, topk: int) -> np.ndarray:
-    """postprocess.py:15-111 with edge='rising', threshold=0, kpsh=False, valley=False, mpd > 1, NaN-free input."""
+    """postprocess.py:15-111 with edge='rising', threshold=0, kpsh=False, valley=False, mpd > 1 (topk None: all)."""
     x = np.asarray(x, dtype=np.float32)
     n = x.size
     if n < 3:
