@@ -31,16 +31,21 @@ from oracle import reference_import as ri  # noqa: E402
 ONLY = set(sys.argv[1:])      # model names and / or "functions": regenerate only these files
 
 
-def fixture(M, name, n, length):
+def fixture(M, name, n, length, sd=None, x=None, tgt=None, ks=(16384, 512, 512)):
+    """The reference's results for model `name`: seeded parameters and inputs (G.synth_state_dict / G.synth_inputs)
+    unless a state dict `sd` and inputs `x`, `tgt` are given.  `ks`: the sample sizes of the outputs, the parameter
+    gradients and the buffers."""
     model = M.create_model(name, in_channels=3, in_samples=length)
     lay = G.layout(model.state_dict())
     blob = torch.load(os.path.join(ri.REF_ROOT, "pretrained", f"{name}_diting.pth"), map_location="cpu")
     assert G.layout(blob.get("model_dict", blob)) == lay              # the shipped checkpoint has this layout
-    sd = G.synth_state_dict(lay)
-    assert G.layout(G.model_state_dict(name, length)) == lay      # load() rebuilds exactly these parameters
+    if sd is None:
+        sd = G.synth_state_dict(lay)
+        assert G.layout(G.model_state_dict(name, length)) == lay      # load() rebuilds exactly these parameters
     model.load_state_dict(sd, strict=True)
     ri.zero_drop_rates(model)
-    x, tgt = G.synth_inputs(name, n, length)
+    if x is None:
+        x, tgt = G.synth_inputs(name, n, length)
     model.eval()
     with torch.no_grad():
         y_eval = model(x)
@@ -56,10 +61,10 @@ def fixture(M, name, n, length):
     out = {
         "model": name, "batch": n, "length": length, "layout_sha": G.digest(lay),
         "param_sha": G.digest([k for k, _ in model.named_parameters()]),
-        "y_shape": tuple(y_eval.shape), "y_eval": G.pack([y_eval], 16384, seed=1), "y_train": G.pack([y_train], 16384, seed=2),
+        "y_shape": tuple(y_eval.shape), "y_eval": G.pack([y_eval], ks[0], seed=1), "y_train": G.pack([y_train], ks[0], seed=2),
         "loss": loss.detach(),
-        "grads": G.pack([p.grad for _, p in model.named_parameters()], 512, seed=1000),
-        "buffers_after": G.pack([b for _, b in model.named_buffers()], 512, seed=3000),
+        "grads": G.pack([p.grad for _, p in model.named_parameters()], ks[1], seed=1000),
+        "buffers_after": G.pack([b for _, b in model.named_buffers()], ks[2], seed=3000),
     }
     if name.endswith("dpk"):
         det = y_eval[:, 0]

@@ -40,6 +40,7 @@ from seist_b200.plan import ACT_GELU, OUT_SIGMOID
 
 NAME, N, L = "seist_m_dpk", 512, 8192       # bench.py's flagship workload
 SM_COUNT = 132                              # H100 SXM
+AT_SCALE_SEED = 7                           # oracle/pretrained.inputs seed of the checkpoint cases at production shapes
 TOL = 2e-4
 D = torch.float64
 
@@ -54,15 +55,18 @@ CHAN_TOL = {
     ("att_bwd_q", "grad"): 3e-5,                          # 1.72e-5 (baz)
     ("att_fwd", "out"): 1e-5,                             # 2.75e-6 (l)
     ("bww(simt)", "dW"): 3e-7,                            # 7.80e-8 (baz)
-    ("bww(simt)", "dbias"): 1e-7,                         # 8.46e-8 (baz; 2.45e-8 at the bench shape)
-    ("bwwk(simt)", "dW"): 1e-7,                           # 5.05e-8 (baz)
+    ("bww(simt)", "dbias"): 7e-7,                         # 1.34e-7 (m_dpk checkpoint, fine-tuning; 8.46e-8 baz
+                                                          # seeded): a 4.2 M-term sum, rounding up to ~1e-4
+    ("bwwk(simt)", "dW"): 1.5e-6,                         # 2.52e-7 (m_dpk checkpoint, fine-tuning; 5.05e-8 baz
+                                                          # seeded): a 4.2 M-term sum, rounding up to ~1e-4
     ("bwwk(simt)", "dbias"): 3e-8,                        # 6.65e-9 (l)
     ("conv_bwd_data(simt)", "grad"): 1.5e-6,              # 2.89e-7 (ragged)
     ("conv_bwd_data(simt)", "gstat"): 5e-8,               # 1.07e-8 (ragged)
     ("conv_fwd(simt)", "out"): 1.5e-6,                    # 2.89e-7 (ragged)
     ("conv_fwd(simt)", "stat"): 2e-7,                     # 3.74e-8 (ragged)
     ("convk_bwd_data(simt)", "grad"): 2e-6,               # 4.08e-7
-    ("convk_bwd_data(simt)", "gstat"): 3e-9,              # 5.88e-10
+    ("convk_bwd_data(simt)", "gstat"): 1.5e-8,            # 3.11e-9 (m_dpk checkpoint, fine-tuning; 5.88e-10
+                                                          # seeded): a 4.2 M-term statistic sum
     ("convk_fwd(simt)", "out"): 2e-6,                     # 3.63e-7
     ("convk_fwd(simt)", "stat"): 7e-8,                    # 1.41e-8
     ("headvec_bwd", "dW"): 3.5e-6,                        # 6.86e-7 (baz)
@@ -82,8 +86,13 @@ CHAN_TOL = {
     ("stem_compose_fwd", "W_eff"): 7e-7,                  # 1.66e-7
     ("tcconv_bwd_data(wgmma+TMA)", "grad"): 5e-6,         # 1.04e-6 (baz)
     ("tcconv_bwd_data(wgmma+TMA)", "gstat"): 5e-8,        # 1.34e-8 (baz)
-    ("tcconv_fwd(wgmma+TMA)", "out"): 7e-6,               # 1.42e-6 (l)
-    ("tcconv_fwd(wgmma+TMA)", "stat"): 2e-6,              # 4.88e-7
+    ("tcconv_fwd(wgmma+TMA)", "out"): 5e-5,               # 9.27e-6 (l_dpk checkpoint, eval, the first up-sampled
+                                                          # head conv; 1.42e-6 l seeded): its input's BatchNorm is
+                                                          # applied in fp32 as x * scale + shift, whose rounding
+                                                          # scales with |x * scale| + |shift|, up to ~8.6x |BN(x)|
+                                                          # with the trained running means, not with |BN(x)|
+    ("tcconv_fwd(wgmma+TMA)", "stat"): 1.3e-5,            # 2.56e-6 (m_dpk checkpoint, fine-tuning, SEIST_TCC=1;
+                                                          # 4.88e-7 seeded): a 4.2 M-term statistic sum
 }
 
 
@@ -386,17 +395,20 @@ def _calibrated_state(name, length, steps=40):
     return {k: v.detach().cpu() for k, v in m.state_dict().items()}
 
 
-def run_at_scale(name, n, length, training, drops=None, step_seed=12345):
+def run_at_scale(name, n, length, training, drops=None, step_seed=12345, state_dict=None, x=None):
     """Runs every op of the plan on the kernels and on the float64 interpreter; returns the _Report.  `drops`: the
-    drop rates (None: no dropout); `step_seed`: the dropout step counter, an unsigned 64-bit value."""
-    sd = None if training else _calibrated_state(name, length)
+    drop rates (None: no dropout); `step_seed`: the dropout step counter, an unsigned 64-bit value; `state_dict`: the
+    parameters and running statistics (None: harness.randomize, calibrated in eval); `x`: the (n, 3, length) input
+    (None: seeded white noise)."""
+    sd = state_dict if state_dict is not None else (None if training else _calibrated_state(name, length))
     p_ref, p_gpu, it, _, _ = build_pair(name, n, length, training, drops=drops, ref_device="cuda", ref_dtype=D,
                                         state_dict=sd)
     rep = _Report()
     rep.sites = dropout_sites(p_ref)
     g = torch.Generator().manual_seed(1)
     p_ref.step_seed.fill_(step_seed - (1 << 64) if step_seed >> 63 else step_seed)     # int64 holds the same bits
-    p_ref.x_in.x.copy_(torch.randn(n, 3, length, generator=g))
+    xn = torch.randn(n, 3, length, generator=g)       # drawn either way: the output gradient below stays the same
+    p_ref.x_in.x.copy_(xn if x is None else x)
     p_ref.stat.zero_()
 
     for i, (fr, fg, fam) in enumerate(zip(p_ref.fwd_ops, p_gpu.fwd_ops, _families(p_gpu.c_fwd))):
@@ -525,16 +537,17 @@ def _release():
     torch.cuda.empty_cache()
 
 
-def check_at_scale(name, n, length, training, drops=None, step_seed=12345):
+def check_at_scale(name, n, length, training, drops=None, step_seed=12345, state_dict=None, x=None, label=""):
     """run_at_scale on one configuration; prints the worst per-channel ratio of every (family, quantity) it reached and
     fails on any whole-tensor or per-channel failure, or on a dropout site that was not held to the per-channel
-    criterion."""
+    criterion.  `label` names the parameters and inputs in the printout."""
     t0 = time.time()
     try:
-        rep = run_at_scale(name, n, length, training, drops, step_seed)
+        rep = run_at_scale(name, n, length, training, drops, step_seed, state_dict, x)
     finally:
         _release()
     print(f"\n{name} N={n} L={length} training={training} SEIST_TCC={os.environ.get('SEIST_TCC', '')}"
+          + (f" {label}" if label else "")
           + (f" drops={drops} step_seed={step_seed}" if drops is not None else "") +
           f": {time.time() - t0:.0f} s; {rep.pool_ties} max-pool near ties left out; "
           + (f"{len(rep.sites)} dropout sites; " if rep.sites else "") + "worst per-channel error / magnitude by family:")
@@ -547,13 +560,17 @@ def check_at_scale(name, n, length, training, drops=None, step_seed=12345):
     return rep
 
 
-def check_on_tensor_cores(name, n, length, families=("tcconv_bwd",), drops=None, step_seed=12345):
+def check_on_tensor_cores(name, n, length, families=("tcconv_bwd",), drops=None, step_seed=12345, pretrained=False):
     """check_at_scale in a child process with SEIST_TCC=1 (read once per process): every eligible forward /
-    data-gradient conv runs on the persistent wgmma engine.  Each of `families` must prefix a family that ran."""
+    data-gradient conv runs on the persistent wgmma engine.  Each of `families` must prefix a family that ran.
+    `pretrained`: the child loads the shipped checkpoint of `name` and runs it on event inputs
+    (oracle/pretrained.py)."""
     _release()
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = ("import sys; sys.path.insert(0, 'tests'); import test_gpu_ops_at_scale as T;"
-            f"rep = T.check_at_scale({name!r}, {n}, {length}, True, {drops!r}, {step_seed});"
+    args = (f"state_dict=PT.pretrained_state_dict({name!r}), x=PT.inputs({name!r}, {n}, {AT_SCALE_SEED}), "
+            "label='pretrained'") if pretrained else ""
+    code = ("import sys; sys.path.insert(0, 'tests'); import test_gpu_ops_at_scale as T; from oracle import pretrained as PT;"
+            f"rep = T.check_at_scale({name!r}, {n}, {length}, True, {drops!r}, {step_seed}, {args});"
             f"missing = [p for p in {tuple(families)!r} if not any(f.startswith(p) for f, _ in rep.worst)];"
             "assert not missing, ('no op of these families ran', missing);"
             "print('TC-OK')")
