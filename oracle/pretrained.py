@@ -105,9 +105,9 @@ def record(kind, g, length=RECORD):
     return x, p, s
 
 
-def _records(n, seed, kinds):
+def _records(n, seed, kinds, length=RECORD):
     g = torch.Generator().manual_seed(seed)
-    return [record(kinds[i % len(kinds)], g) for i in range(n)]
+    return [record(kinds[i % len(kinds)], g, length) for i in range(n)]
 
 
 def dpk_windows(n=DPK_N, seed=DPK_SEED):
@@ -120,6 +120,13 @@ def dpk_windows(n=DPK_N, seed=DPK_SEED):
         ts.append(PR.dpk_labels(ps, ss, WINDOW, LABEL_WIDTH, LABEL_SHAPE, CODA_RATIO))
         phases.append((p, s))
     return torch.from_numpy(np.stack(xs)), torch.from_numpy(np.stack(ts)), phases
+
+
+def dpk_records(n=DPK_N, seed=DPK_SEED, length=RECORD):
+    """(n, 3, length) float32: the whole records of `dpk_windows` (row i of kind KINDS[i % 8]; the same records at the
+    default length), each normalised "std" as one window of `length` samples."""
+    return torch.from_numpy(np.stack([PR.normalize(rec.numpy().astype(np.float32), MODE)
+                                      for rec, _, _ in _records(n, seed, KINDS, length)]))
 
 
 EVENT_KINDS = tuple(k for k in KINDS if k != "noise")

@@ -1,8 +1,11 @@
 // Attention core of AttentionBlock (reference models/seist.py:381-388):
 //   out[n, h*E+e, l] = sum_j softmax_j( (q[n,h,:,l]/sqrt(E)) . k[n,h,:,j] ) * v[n,h,e,j]
-// q is (N, C, Lq), k/v are (N, C, Lk) with Lk = Lq / attn_aggr_ratio (128 for L = 8192 at every stage),
-// so K and V of one (waveform, head) — at most 2 x 32 x 128 floats — sit in shared memory and each
-// thread owns one query column in registers (flash-style online softmax, no (Lq x Lk) matrix in HBM).
+// q is (N, C, Lq), k/v are (N, C, Lk) with Lk = Lq / attn_aggr_ratio = L / 64 at every stage: 128 for L = 8192,
+// 157 for 10000, 256 for 16384 (the longest window preprocess and pick_phase accept).  K and V of one (waveform,
+// head) are staged through shared memory KV_CHUNK keys at a time — at most 2 x 32 x 128 floats, one chunk up to
+// L = 8192, two past it — and each thread owns one query column in registers (flash-style online softmax carried
+// across the chunks, no (Lq x Lk) matrix in HBM).  tests/test_gpu_attention.py checks all three kernels across
+// chunk boundaries against float64.
 // Lanes run along the sample axis: every global access is a coalesced channel-row segment.
 #include "common.cuh"
 
