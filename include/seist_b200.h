@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define SEIST_ABI_VERSION 23
+#define SEIST_ABI_VERSION 24
 #define SEIST_MAX_IN 3
 
 /* ---- BatchNorm table entry (nn.BatchNorm1d, models/seist.py:641; SURVEY §3.5) ---------------- */
@@ -577,11 +577,33 @@ int seist_gap_stream_copy(const float* src, int64_t src_capacity, const int64_t*
                            call writes outputs K0 .. K0 + m_s - 1 (m_s = out_off[s + 1] - out_off[s]) as a (C, m_s) block at
                            C * out_off[s] of out, and inputs lo1 .. N0 + n_s - 1 to held_out row (s, c) (distinct from held).
                            Those outputs must have all their in-record inputs among lo0 .. N0 + n_s - 1; max_m >= every m_s sizes
-                           the grid.  One launch; a malformed descriptor gives wrong output but no out-of-range access. */
+                           the grid.  One launch; a malformed descriptor gives wrong output but no out-of-range access.
+   Stations of different ratios share one launch through a filter table (DESIGN §4.24):
+   seist_resample_table        = host only: fills table (F, 8) int32, one row per distinct reduced ratio i: up, down, hl, nt,
+                                 tap_off, tile, identity, smem.  up == down gives the identity row (hl = nt = 0, no taps: the
+                                 outputs are the inputs, copied bit for bit); otherwise the filter above.  tap_off is where
+                                 the row's up * nt taps start in the concatenated taps (each padded to 4 floats), tile the
+                                 outputs one CTA computes and smem the dynamic shared bytes such a CTA needs.
+   seist_resample_multi        = whole records of S stations of C channels into out (S, C, T_max): desc is a device int64
+                                 array of src (the device address of station s's (C, T_s) record), T_s, filt (the table row
+                                 of station s) (S each), then cta_off (S + 1).  Row (s, c) holds ceil(T_s * up / down)
+                                 outputs, then NaN up to T_max.  Station s owns CTAs cta_off[s] .. cta_off[s + 1] - 1, C * n_s
+                                 of them: per channel ceil(T_out_s / tile) output tiles, then the rest fill the NaN tail in
+                                 equal shares.  ctas = cta_off[S] sizes the grid and smem >= every smem of the rows used.
+   seist_resample_multi_stream = seist_resample_stream with a filter per station: desc continues with filt (S) and cta_off
+                                 (S + 1), station s owning C * max(1, ceil(m_s / tile)) CTAs; held is (S, C, H).
+   One launch each, no host synchronisation; a malformed descriptor, table index or smem gives wrong output but no
+   out-of-range access beyond the records desc points to. */
 int seist_resample(const float* record, int32_t rows, int64_t T, const float* taps, int32_t up, int32_t down, float* out, void* stream);
 int seist_resample_stream(const float* held, int64_t H, const float* chunk, int64_t chunk_capacity, const int64_t* desc, int32_t S,
                           int32_t C, int64_t max_m, const float* taps, int32_t up, int32_t down, float* out, int64_t out_capacity,
                           float* held_out, void* stream);
+int seist_resample_table(int32_t F, const int32_t* up, const int32_t* down, int32_t* table);
+int seist_resample_multi(const int64_t* desc, int32_t S, int32_t C, int64_t T_max, int64_t ctas, const int32_t* table, int32_t F,
+                         int32_t smem, const float* taps, float* out, void* stream);
+int seist_resample_multi_stream(const float* held, int64_t H, const float* chunk, int64_t chunk_capacity, const int64_t* desc,
+                                int32_t S, int32_t C, int64_t ctas, const int32_t* table, int32_t F, int32_t smem, const float* taps,
+                                float* out, int64_t out_capacity, float* held_out, void* stream);
 
 /* *seed += 1 (device scalar), keeps dropout streams distinct across graph replays */
 int seist_advance_seed(uint64_t* seed, void* stream);

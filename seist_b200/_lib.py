@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libseist_b200.so")
-ABI_VERSION = 23
+ABI_VERSION = 24
 MAX_IN = 3
 MAX_WORLD = 8
 SIG_LANES = 4
@@ -272,6 +272,12 @@ def lib():
     L.seist_resample.argtypes = [P, I32, I64, P, I32, I32, P, P]
     L.seist_resample_stream.restype = C.c_int
     L.seist_resample_stream.argtypes = [P, I64, P, I64, P, I32, I32, I64, P, I32, I32, P, I64, P, P]
+    L.seist_resample_table.restype = C.c_int
+    L.seist_resample_table.argtypes = [I32, P, P, P]
+    L.seist_resample_multi.restype = C.c_int
+    L.seist_resample_multi.argtypes = [P, I32, I32, I64, I64, P, I32, I32, P, P, P]
+    L.seist_resample_multi_stream.restype = C.c_int
+    L.seist_resample_multi_stream.argtypes = [P, I64, P, I64, P, I32, I32, I64, P, I32, I32, P, P, I64, P, P]
     L.seist_sizeof_comm.restype = C.c_uint64
     L.seist_comm_barrier.restype = C.c_int
     L.seist_comm_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
@@ -313,7 +319,7 @@ EXPORTS = [
     "seist_segment_gather", "seist_segment_event_windows",
     "seist_gap_stream_scan", "seist_gap_stream_fill", "seist_gap_stream_pack", "seist_gap_stream_copy",
     "seist_gap_event_windows",
-    "seist_resample", "seist_resample_stream",
+    "seist_resample", "seist_resample_stream", "seist_resample_table", "seist_resample_multi", "seist_resample_multi_stream",
 ]
 
 
